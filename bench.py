@@ -10,7 +10,8 @@ Workload (configs[1] of BASELINE.json, fits one GPU): 1920x1080, 4 sub-samples p
 NEE with 5 candidates + 1 shadow ray per vertex, Russian roulette, firefly filter on, environment map on, on the ~2.8 M triangle procedural
 "city block" stand-in for Bistro exterior (the real Bistro assets are git-LFS stubs in the reference tree: SURVEY.md F7).
 A step is one frame: 4 sub-samples path traced and folded into the accumulation buffer.  A ray is one traversal query (scatter or shadow).
-One JSON line on stdout (rank 0).
+One JSON line on stdout (rank 0).  --dump-outputs DIR writes what the last timed step computed (rank 0's accumulated RGBA32F frame) as DIR/accumulated.npy; the
+inputs are fixed by the arguments, so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -45,7 +46,7 @@ def workload_config(n_gpus):
                         % (WIDTH, HEIGHT, SPP, BOUNCES, BOUNCES),
             "triangles": TARGET_TRIANGLES, "materials": 254, "image": [WIDTH, HEIGHT], "spp_per_frame": SPP,
             "partition": "1 GPU, whole frame" if n_gpus == 1 else "interleaved 64x64 screen tiles over %d GPUs + NCCL all-gather of radiance tiles" % n_gpus,
-            "cache": "working set per frame (path state 664 MB + scene ~400 MB) exceeds the 126 MB L2; no explicit flush"}
+            "cache": "working set per frame (path state 664 MB + scene ~400 MB) exceeds the 50 MB L2; no explicit flush"}
 
 
 def _gpu_uuid(torch, index):
@@ -55,20 +56,22 @@ def _gpu_uuid(torch, index):
 
 
 class ClockSampler:
-    """SM clock, power and clock-event reasons of this rank's GPU sampled DURING the timed region (B200_PROFILING.md clocks line).  NVML in a thread of this process (what
-    nvidia-smi itself reads): a looping `nvidia-smi -lms` process needed 70-100+ ms per query on the 8-GPU boxes and held the driver while it enumerated the node - the N=8 timed
-    loop of round 1 / early round 2 measured 6.7 ms per frame against 3.6 ms for the same frames with a host synchronize in between, with ONE clock sample taken
-    (profiles/r2_history.md section 10).  Falls back to nvidia-smi when NVML cannot be loaded."""
+    """SM clock, power and clock-event reasons of this rank's GPU sampled DURING the timed region.  NVML in a thread of this process (what nvidia-smi itself reads): a looping
+    `nvidia-smi -lms` process can need tens of milliseconds per query on a many-GPU node and holds the driver while it enumerates the node, which slows the timed frames it
+    samples.  Falls back to nvidia-smi when NVML cannot be loaded."""
     REASONS = (("hw_slowdown", "HwSlowdown"), ("hw_thermal_slowdown", "HwThermalSlowdown"), ("sw_thermal_slowdown", "SwThermalSlowdown"), ("sw_power_cap", "SwPowerCap"))
 
     def __init__(self, index, uuid=None, period_s=0.01):
         self.sm, self.mx, self.reasons, self.proc, self.nvml, self.stop_flag, self.lines, self.source = [], [], set(), None, None, False, [], "nvml"
+        self.power_limit_w = None
         try:
             import pynvml
             pynvml.nvmlInit(); self.nvml = pynvml
             try: self.handle = pynvml.nvmlDeviceGetHandleByUUID(uuid if isinstance(uuid, bytes) else str(uuid).encode()) if uuid else pynvml.nvmlDeviceGetHandleByIndex(index)
             except Exception: self.handle = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.max_sm = float(pynvml.nvmlDeviceGetMaxClockInfo(self.handle, pynvml.NVML_CLOCK_SM)); self.period = period_s
+            try: self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(self.handle) / 1000.0
+            except Exception: pass      # some virtualised / MIG setups refuse the query; the clock samples do not depend on it
             self.thread = threading.Thread(target=self._poll, daemon=True); self.thread.start()
             return
         except Exception:
@@ -103,7 +106,8 @@ class ClockSampler:
     def stop(self):
         if self.nvml is not None:
             self.stop_flag = True; self.thread.join(1.0)
-            return {"sm_mhz": float(np.median(self.sm)) if self.sm else None, "sm_max_mhz": max(self.mx) if self.mx else None, "reasons": sorted(self.reasons), "samples": len(self.sm), "source": "nvml"}
+            return {"sm_mhz": float(np.median(self.sm)) if self.sm else None, "sm_max_mhz": max(self.mx) if self.mx else None, "reasons": sorted(self.reasons), "samples": len(self.sm), "source": "nvml",
+                    "power_limit_w": self.power_limit_w}
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
@@ -127,50 +131,19 @@ def measured_peak_gbs():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_capture(rays_per_iteration):
-    """Counters of k_trace_closest from the committed `ncu --set full` capture (profiles/r2_ncu_full_summary.json, else round 1's): DRAM bytes per frame, the share of issue
-    slots in use and the executed thread-instructions per ray.  The capture holds the launches of the first iterations of one frame; byte and instruction totals are scaled to
-    the frame by this run's ray counts (same unit as `achieved`: per frame = per launch x launches).  The numbers describe the build the capture was taken from: its commit is
-    reported next to them, and a capture older than the kernels goes stale - `traffic_note` says which file was read."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    for name in ("r2_ncu_full_summary.json", "r1_ncu_full_summary.json"):
-        path = os.path.join(here, "profiles", name)
-        if not os.path.exists(path):
-            continue
-        try:
-            data = json.load(open(path)); rows_all = data["rows"] if isinstance(data, dict) else data
-            rows = [r for r in rows_all if "k_trace_closest" in r["kernel"]]
-            captured = sum(r["dram_read_bytes"] + r["dram_write_bytes"] for r in rows)
-            frac = sum(rays_per_iteration[:len(rows)]) / max(1, sum(rays_per_iteration))
-            rays_captured = sum(rays_per_iteration[:len(rows)])
-            ms = sum(r["time_ms"] for r in rows)
-            out = {"traffic": captured / frac, "capture_ms": ms, "capture_dram_bytes": captured,
-                   # time-weighted over the captured launches (the last bounces are a few microseconds at single-digit utilisation: a plain mean would describe them)
-                   "issue_active": float(sum(r["issue_active_pct"] * r["time_ms"] for r in rows) / max(ms, 1e-9)) / 100.0 if "issue_active_pct" in rows[0] else None,
-                   "threads_per_inst": float(sum(r["threads_per_inst"] * r["time_ms"] for r in rows) / max(ms, 1e-9)) if "threads_per_inst" in rows[0] else None,
-                   "thread_inst_per_ray": (sum(r["warp_insts"] * r["threads_per_inst"] for r in rows) / max(1, rays_captured)) if "warp_insts" in rows[0] else None,
-                   "commit": data.get("commit") if isinstance(data, dict) else "round 1 (e38f795 or earlier)",
-                   "note": "profiles/%s: %d captured launches = %.0f %% of the frame's scatter rays, scaled to the frame" % (name, len(rows), 100 * frac)}
-            return out
-        except Exception as e:  # malformed capture: say so instead of guessing
-            return {"traffic": None, "note": "capture %s unreadable (%s)" % (name, e)}
-    return {"traffic": None, "note": "no ncu capture committed under profiles/"}
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def cpu_sample_rect():
     # bounded sample of the same workload: a 960x540 window in the middle of the 1080p frame, 1 sub-sample (~2.4 M rays per step: enough rows to keep
-    # every host thread busy, about a second per step on 64 cores)
+    # every host thread busy)
     w, h = 960, 540
     x0, y0 = (WIDTH - w) // 2, (HEIGHT - h) // 2
     return x0, y0, x0 + w, y0 + h
 
 
 def physical_cores():
-    """Host threads the CPU arm uses: one per physical core the process may run on (SMT siblings only slow the BVH-walking oracle down:
-    measured 5.5 Mrays/s on 64 threads vs 3.2 on 128 on the GPU box)."""
+    """Host threads the CPU arm uses: one per physical core the process may run on (SMT siblings slow the BVH-walking oracle down)."""
     try:
         allowed = os.sched_getaffinity(0); cores = set(); cur = {}
         for line in open("/proc/cpuinfo"):
@@ -215,7 +188,10 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-realtime", action="store_true", help="skip the realtime-mode (stable planes) timing that runs in a child process after the headline measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the accumulated frame of the last timed step as DIR/accumulated.npy (float32, HxWx4)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be at least 1 and --warmup at least 0")
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     n_gpus = args.gpus
 
@@ -300,6 +276,10 @@ def main():
         rays_per_frame = float(rays_per_frame_local)
     clocks = sampler.stop() if sampler else None
     ms_per_step = ms_total / args.steps
+    if args.dump_outputs and rank == 0:
+        # after the last timed step the accumulation buffer holds its result (N > 1: the whole frame, every rank's tiles unpacked); the e2e frames below add to it
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "accumulated.npy"), ctx.readback_accumulated(np.empty((HEIGHT, WIDTH, 4), np.float32)))
     value = rays_per_frame / (ms_per_step * 1e-3) / 1e6
 
     # ---- where a frame's time goes on this rank (N > 1: the scaling curve's explanation): CUDA events between the phases of 6 further frames, max over ranks per phase ------
@@ -358,16 +338,10 @@ def main():
         alg_bytes = 48 * s2.scatterRays + 80 * s2.traversalNodeVisits + 48 * s2.traversalTriTests      # SURVEY.md §8d: 32 B ray in + 16 B hit out + 80 B/node + 48 B/triangle
         peak, peak_src = measured_peak_gbs()
         achieved = alg_bytes / (k_closest * 1e-3) / 1e9 if k_closest > 0 else 0.0
-        cap = ncu_capture(rays_per_bounce)
-        dram_gbs = (cap["capture_dram_bytes"] / (cap["capture_ms"] * 1e-3) / 1e9) if cap.get("capture_ms") else None
-        # The traversal kernel is bound by instruction issue, not by HBM (profiles/): `frac` stays the contract's algorithmic-bytes figure (SURVEY §8d: what the kernel would
-        # have to move if nothing were cached, over its time and the measured HBM peak); `frac_dram` is what ncu saw cross the DRAM interface, `issue_active` the share of
-        # issue slots in use - the number the kernel is actually limited by - and `thread_inst_per_ray` the quantity to drive down.
-        roofline = {"kernel": "k_trace_closest (CWBVH8 closest-hit traversal)", "bound": "issue", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "frac_basis": "algorithmic bytes (48 B/ray + 80 B/node visit + 48 B/triangle test) / kernel time / measured HBM peak",
-                    "traffic": cap.get("traffic"), "traffic_note": cap.get("note"), "traffic_capture_commit": cap.get("commit"),
-                    "frac_dram": (dram_gbs / peak) if dram_gbs else None, "dram_gbs": dram_gbs,
-                    "issue_active": cap.get("issue_active"), "threads_per_inst": cap.get("threads_per_inst"), "thread_inst_per_ray": cap.get("thread_inst_per_ray"),
+        # `frac`: the algorithmic bytes (SURVEY §8d: what the kernel would have to move if nothing were cached) over its time and the HBM peak.  Above 1 the nodes and
+        # triangles are served from L1 / L2, i.e. the kernel is not bound by HBM bandwidth.
+        roofline = {"kernel": "k_trace_closest (CWBVH8 closest-hit traversal)", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
+                    "frac_basis": "algorithmic bytes (48 B/ray + 80 B/node visit + 48 B/triangle test) / kernel time / HBM peak",
                     "peak_source": peak_src,
                     "algorithmic_bytes_per_frame": int(alg_bytes), "nodes_per_ray": s2.traversalNodeVisits / max(1, s2.scatterRays), "tris_per_ray": s2.traversalTriTests / max(1, s2.scatterRays),
                     "kernel_ms_per_frame": {"trace_closest": k_closest, "trace_shadow": k_shadow, "shade": k_shade, "other": k_other},
@@ -393,7 +367,7 @@ def main():
     if rank == 0:
         line = {"metric": "Mrays/s", "value": value, "unit": "Mrays/s", "n_gpus": n_gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step,
                 "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32 (fp16 path-state storage)", "data": "synthetic",
-                "config": workload_config(n_gpus),
+                "device": torch.cuda.get_device_name(local_rank), "config": workload_config(n_gpus),
                 "e2e": {"value": e2e_value, "unit": "Mrays/s", "h2d_bytes_per_step": C.sizeof(type(consts)), "d2h_bytes_per_step": WIDTH * HEIGHT * 16,
                         "ms_per_step": float(e2e_t[0]) / args.steps * 1e3},
                 "gpu_launches": int(launches * args.steps),

@@ -1,5 +1,5 @@
 /*
- * rtxpt_b200.h — C ABI of the B200-native wavefront path tracer that drops in for RTXPT's single
+ * rtxpt_b200.h — C ABI of the CUDA-native (H100, sm_90a) wavefront path tracer that drops in for RTXPT's single
  * PathTrace dispatch.
  *
  * Every entry point below replaces one piece of the reference's host→GPU boundary for that path.  The

@@ -62,7 +62,7 @@ struct rtxpt_ctx
     // scene
     bool haveScene = false, haveConstants = false, lightsDirty = true; uint64_t lightVersion = 0;       // bumped by every re-bake of the light list (uploadLights)
     size_t l2PersistBytes = 0, l2WindowMax = 0;
-    // measurement knobs, read from the environment once at creation (defaults are the measured optimum on B200, profiles/r1_history.md)
+    // measurement knobs, read from the environment once at creation (RTXPT_* variables; the defaults measured fastest on an H100 SXM at a 400 W power limit, bench.py workload: see the launch configuration)
     struct Tuning { int refillThreshold = 24, waitFlushLanes = 8, traceCtas = 4, shadeCtas = 4, smemNodes = 0, lanes = 1, shadowLpt = 1; } tune; float sceneDiagonal = 0;
     cudaStream_t stream2 = nullptr; cudaEvent_t evShadeDone = nullptr, evShadowDone = nullptr; bool overlapShadow = true;
     // pipeline lanes: the sub-samples of one launch are split into independent wavefronts, each on its own pair of streams, so that the latency-bound tail of every
@@ -204,7 +204,7 @@ extern "C" RTXPT_API int rtxpt_b200_create(const RtxptConfig* config, rtxpt_ctx*
     c->tune.refillThreshold = envInt("RTXPT_REFILL_THRESHOLD", 24, 1, 32); c->tune.waitFlushLanes = envInt("RTXPT_WAIT_FLUSH", 8, 1, 33);
     c->tune.traceCtas = envInt("RTXPT_TRACE_CTAS", 4, 2, 4); c->tune.shadeCtas = envInt("RTXPT_SHADE_CTAS", 4, 3, 5); c->tune.smemNodes = envInt("RTXPT_SMEM_NODES", 0, 0, 1 << 20);
     c->tune.shadowLpt = envInt("RTXPT_SHADOW_LPT", 1, 0, 1);
-    c->tune.lanes = envInt("RTXPT_LANES", 1, 1, rtxpt_ctx::kMaxLanes);          // measured on a B200, 1080p 4 spp: 1 lane 18.61 ms, 2 lanes 18.79, 4 lanes 19.51 (one GPU has enough rays per wavefront; lanes are for small per-rank tile sets)
+    c->tune.lanes = envInt("RTXPT_LANES", 1, 1, rtxpt_ctx::kMaxLanes);          // H100 (400 W), bench.py, ms/frame: 1 lane 25.4-25.5, 2 lanes 25.8 (one GPU has enough rays per wavefront; lanes are for small per-rank tile sets)
     cudaEventCreateWithFlags(&c->evFork, cudaEventDisableTiming);
     for (int l = 1; l < rtxpt_ctx::kMaxLanes; l++) { cudaStreamCreateWithFlags(&c->lanes[l].s, cudaStreamNonBlocking); cudaStreamCreateWithFlags(&c->lanes[l].s2, cudaStreamNonBlocking); }
     for (int l = 0; l < rtxpt_ctx::kMaxLanes; l++) { cudaEventCreateWithFlags(&c->lanes[l].evShadeDone, cudaEventDisableTiming); cudaEventCreateWithFlags(&c->lanes[l].evShadowDone, cudaEventDisableTiming); cudaEventCreateWithFlags(&c->lanes[l].evCommitted, cudaEventDisableTiming); }
@@ -646,13 +646,12 @@ static void fillParams(rtxpt_ctx* c, LaunchParams& p)
     memcpy(p.worldToClip, c->worldToClip, sizeof(p.worldToClip)); p.exportGuides = ((c->cfg.flags & RTXPT_CFG_EXPORT_GUIDES) && c->haveView) ? 1u : 0u;
     // traversal occupancy and the shared-memory BVH prefix are chosen together: B resident CTAs of 256 threads per SM (register budget
     // 65536 / (256 B): 128 / 85 / 64 registers for B = 2 / 3 / 4) share the 227 KB of shared memory
-    const int blocks = c->tune.traceCtas;       // measured on B200 (city workload, ms/frame closest+shadow): 2 CTAs 28.5, 3 CTAs 21.3, 4 CTAs 19.1
+    const int blocks = c->tune.traceCtas;       // H100 (400 W), bench.py, ms/frame: 4 CTAs 25.4-25.5, 3 CTAs 26.7; shade CTAs (RTXPT_SHADE_CTAS): 3 25.6, 4 25.4-25.5, 5 27.3
     c->grid.traceBlocksPerSM = blocks;
     c->grid.shadeBlocksPerSM = c->tune.shadeCtas;
     const uint32_t budget = uint32_t(std::max(0, std::min(c->maxSmemOptin, (227 * 1024) / blocks - 2048) - 1024 - 8 * 2320));     // 8 x WarpScratch (traverse.cuh)
-    // BVH prefix (breadth-first top levels) staged into shared memory by TMA.  Measured on B200 (city workload, closest+shadow ms/frame):
-    // 0 nodes 14.04, 73 nodes 14.36, 200 nodes 14.37, as many as fit (~450) 14.71 - shared memory taken from the unified L1 costs more than the
-    // staged levels save, so the default is 0 and RTXPT_SMEM_NODES opts in.
+    // BVH prefix (breadth-first top levels) staged into shared memory by TMA: shared memory taken from the unified L1 costs the node and triangle
+    // loads that miss the staged levels (H100 SXM, 700 W, bench.py: 200 staged nodes 23.72 ms/frame, none 23.16-23.18), so the default is 0 and RTXPT_SMEM_NODES opts in.
     // optional: keep the BVH nodes in the persisting part of L2 (RTXPT_L2_PERSIST_MB > 0) while path state streams through
     c->grid.l2WindowBase = nullptr; c->grid.l2WindowBytes = 0;
     if (c->l2PersistBytes && c->dBvhNodes.ptr) { c->grid.l2WindowBase = c->dBvhNodes.ptr; c->grid.l2WindowBytes = std::min(size_t(c->bvhNodeCount) * 80, c->l2WindowMax); c->grid.l2WindowHitRatio = std::min(1.0f, float(c->l2PersistBytes) / float(c->grid.l2WindowBytes)); }

@@ -1,6 +1,6 @@
 // envbake_kernels.cu - EnvMapBaker's BaseLayerCS and MIPReduceCS over the bodies in envbake.cuh: one thread per half-resolution texel and face, 8x8 CTAs as the reference
 // dispatches them.  A bake is a once-per-environment-change job (a 2048 cube: 25 M source taps, ~0.5 GB written), bound by the transcendental maths of the direction / solid
-// angle functions rather than by HBM.  First run on a B200 in round 2 (tests/test_gpu_envbake.py); the bodies also pass tests/test_envbake.py on the CPU.
+// angle functions rather than by HBM.  Tested on the GPU by tests/test_gpu_envbake.py; the bodies also pass tests/test_envbake.py on the CPU.
 #include "envbake.cuh"
 #include "kernels.h"
 

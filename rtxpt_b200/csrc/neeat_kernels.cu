@@ -3,7 +3,7 @@
 //                  k_na_proxy_fill (one thread per proxy slot, binary search over the offsets)
 //   update end:    k_na_p1a (half resolution), k_na_p1b, k_na_tiles (one 64-thread CTA per tile: 128 keys gathered by 128 lanes' worth of work, bitonic sort in shared memory,
 //                  run lengths), k_na_clear
-// All of it is integer / reservoir bookkeeping bound by HBM traffic (a few tens of bytes per pixel per pass); grids are sized by the image.  Verified on a B200 in round 2 (tests/test_gpu_neeat.py); the
+// All of it is integer / reservoir bookkeeping bound by HBM traffic (a few tens of bytes per pixel per pass); grids are sized by the image.  Tested on the GPU by tests/test_gpu_neeat.py; the
 // bodies pass tests/test_neeat_port.py on the CPU.
 #include "neeat.cuh"
 #include "kernels.h"

@@ -119,7 +119,8 @@ __global__ void __launch_bounds__(256) k_rt_fill_generate(const __grid_constant_
 
 // ---- shade ------------------------------------------------------------------------------------------------------------------------------------------------------
 #ifndef PT_RT_SHADE_CTAS
-#define PT_RT_SHADE_CTAS 4      // resident CTAs of 128 threads per SM.  Measured on a B200 (config-3 frame, trace ms): 3 CTAs (153-158 registers, no spills) 32.7, 4 CTAs (128 registers, 24-88 B spills) 32.0
+#define PT_RT_SHADE_CTAS 4      // resident CTAs of 128 threads per SM: 4 caps the shade kernels at 128 registers (a few dozen bytes of spills), 3 lets them run without spills.
+                                // H100 SXM (700 W): config-3 trace 41.5 ms/frame with 4, 42.4 with 3; the 1-spp realtime frame 9.69 ms with 4, 9.60 with 3
 #endif
 template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false>
 __global__ void __launch_bounds__(128, PT_RT_SHADE_CTAS) k_rt_shade(const __grid_constant__ LaunchParams p)

@@ -1,7 +1,7 @@
 // reblur_kernels.cu — NRD's REBLUR_DIFFUSE_SPECULAR chain for one stable plane (SURVEY §8 row a18 / K9), one kernel per pass of the dispatch graph
 // (the pass bodies live in reblur_passes.cuh; see there for the per-pass citations).  One thread per pixel, 16x16 CTAs aligned to NRD's 16x16 sky tiles, taps fetched through L2
-// (the working set of one plane at 1080p, ~90 MB, fits the 126 MB L2).  ncu (profiles/r2_ncu_reblur.json) shows every pass bound by instruction issue - ~3600 thread-instructions per
-// pixel per pass, DRAM at 3 % of peak - so tiling pays through the arithmetic it removes (per-tap unpacking, clamped addressing), not through bandwidth: the 5x5 pass stages its
+// (the working set of one plane at 1080p is ~90 MB, larger than the 50 MB L2, so a pass streams its inputs while its taps hit L1 / L2).  The passes are ALU-heavy (thousands
+// of thread-instructions per pixel per pass, a few hundred bytes) - so tiling pays through the arithmetic it removes (per-tap unpacking, clamped addressing), not through bandwidth: the 5x5 pass stages its
 // neighbourhood with TMA (below); the Poisson-tap passes reach up to 40 pixels away and keep reading through L1 / L2.
 #include "reblur_passes.cuh"
 #include "kernels.h"

@@ -1,6 +1,6 @@
 // refit_kernels.cu - rigid-instance animation: k_refit_tris (one thread per leaf triangle: 48 B read of the shade record's positions + 48 B rewrite of the leaf triangle) and
 // k_refit_level (one thread per node of a level, deepest level first, root last: 80 B node + its children's bounds).  HBM-bound streaming passes; the number of level launches
-// is the depth of the 8-wide tree (about log8 of the node count).  Verified on a B200 in round 2 (tests/test_gpu_refit.py: a refitted tree traces like a fresh upload, bit for bit); the bodies also pass tests/test_refit.py on the CPU.
+// is the depth of the 8-wide tree (about log8 of the node count).  Tested on the GPU by tests/test_gpu_refit.py (a refitted tree traces like a fresh upload, bit for bit); the bodies also pass tests/test_refit.py on the CPU.
 #include "refit.cuh"
 #include "kernels.h"
 

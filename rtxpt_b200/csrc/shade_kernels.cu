@@ -27,7 +27,7 @@ PT_DEVICE void warpAppend(uint* queueBase, uint regionStride, uint* counters, ui
     }
 }
 
-// next-item prefetch in k_shade: 0 off, 1 into L2, 2 into L1 (measured: profiles/r2_history.md section 8)
+// next-item prefetch in k_shade: 0 off, 1 into L2, 2 into L1
 #ifndef PT_SHADE_PREFETCH
 #define PT_SHADE_PREFETCH 0
 #endif
@@ -61,7 +61,7 @@ __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ Lau
         const uint count = ctr[kCtrShadeCount + cls];
         const uint* __restrict__ queue = p.wf.shadeQueue + size_t(cls) * p.wf.capacity;
 #if PT_SHADE_PREFETCH
-        // Software pipeline over the queue (the kernel is latency-bound: 4 warps per scheduler, a chain of dependent gathers per path - profiles/r2_history.md section 8): while
+        // Software pipeline over the queue (the kernel is latency-bound: 4 warps per scheduler, a chain of dependent gathers per path): while
         // item k is shaded, the state words and the hit of item k+1 are pulled towards the SM, and once its hit has arrived, its 96-byte shade record.
         uint slotNext = (warpGlobal * 32u + lane < count) ? queue[warpGlobal * 32u + lane] : 0xFFFFFFFFu;
 #endif

@@ -1,5 +1,5 @@
 // skinning_kernels.cu - k_skin_vertices (Donut's skinning_cs: one thread per vertex) and k_skin_gather (one thread per triangle: skinned vertices -> the path tracer's per-triangle
-// shade records).  Streaming passes over one geometry; the BVH refit follows (rtxpt_b200_update_instance_transforms).  Verified on a B200 in round 2 (tests/test_gpu_skinning.py, tests/test_motion_vectors.py).
+// shade records).  Streaming passes over one geometry; the BVH refit follows (rtxpt_b200_update_instance_transforms).  Tested on the GPU by tests/test_gpu_skinning.py and tests/test_motion_vectors.py.
 #include "skinning.cuh"
 #include "kernels.h"
 

@@ -1,5 +1,5 @@
 // tonemap_kernels.cu - luminance reduction (grid-stride accumulation in double, block tree, then one block over the per-block partials: no atomics, deterministic) and the
-// tone-mapping pass (one thread per pixel, RGBA16F or RGBA32F in, SRGBA8 out).  Streaming passes: 8-16 B read + 4 B written per pixel.  Verified on a B200 in round 2 (tests/test_gpu_tonemap.py: byte-identical to the oracle in the IEEE build).
+// tone-mapping pass (one thread per pixel, RGBA16F or RGBA32F in, SRGBA8 out).  Streaming passes: 8-16 B read + 4 B written per pixel.  Tested on the GPU by tests/test_gpu_tonemap.py (byte-identical to the oracle in the IEEE build).
 #include "tonemap.cuh"
 #include "kernels.h"
 
@@ -11,7 +11,7 @@ template <bool F32> PT_DEVICE float4 loadPixel(const void* src, size_t i)
     const uint2 v = reinterpret_cast<const uint2*>(src)[i];
     return make_float4(f16tof32(v.x), f16tof32(v.x >> 16), f16tof32(v.y), f16tof32(v.y >> 16));
 }
-constexpr int kReduceBlocks = 592;      // 148 SMs x 4
+constexpr int kReduceBlocks = 528;      // 132 SMs (H100 SXM) x 4
 template <bool F32>
 __global__ void __launch_bounds__(256) k_tm_luminance(const void* src, uint pixelCount, double* partials)
 {

@@ -114,7 +114,8 @@ struct TraversalCounters { uint nodeVisits, triTests; };
 // byte j of a packed word -> 1 + b * 2^-15, built by placing the byte in mantissa bits 8..15 of 1.0f (one PRMT)
 PT_DEVICE float byteToUnitFloat(uint w, int j) { return __uint_as_float(__byte_perm(w, 0x3F800000u, 0x7604u | (uint(j) << 4))); }
 #ifndef PT_I2F_AXES
-#define PT_I2F_AXES 2       // how many of the three axes convert their bytes with I2F (XU pipe) instead of PRMT (ALU pipe): closest-hit ms/frame 0 axes 9.15, 1 axis 8.98, 2 axes 8.84 (profiles/r1_history.md)
+#define PT_I2F_AXES 2       // how many of the three axes convert their bytes with I2F (XU pipe) instead of PRMT (ALU pipe): 2 spreads the conversions over both pipes.
+                            // H100 SXM (700 W), bench.py ms/frame: 1 axis 23.50, 2 axes 23.16-23.18, 3 axes 23.59
 #endif
 // the same permute with the selector as an immediate: `one` is 0x3F800000 held in a register the compiler cannot see through (otherwise ptxas folds it into the
 // instruction's only immediate slot and spends a second instruction per byte on moving the selector into a register - 16 per node visit in the round-1 SASS)
@@ -131,11 +132,7 @@ PT_DEVICE float byteToUnitFloatImm(uint w, int j, uint one)
     return __uint_as_float(r);
 }
 #ifndef PT_PRMT_IMM
-#define PT_PRMT_IMM 0      // measured on a B200 (closest-hit ms/frame): 8.85 with, 8.81 without - the saved selector moves are re-spent on re-materialising the constant
-#endif
-#ifndef PT_FFMA2
-#define PT_FFMA2 0      // slab test of two children per FFMA2 (Blackwell packed fp32 FMA): 24 instead of 48 FMA issues per node visit, but ptxas pays for the register pairs with
-                        // re-materialised per-node constants at 64 registers: measured on a B200 9.50 ms/frame closest-hit with, 8.81 without (profiles/r2_history.md)
+#define PT_PRMT_IMM 0      // immediate PRMT selectors: the saved selector moves are re-spent on re-materialising the constant (H100 SXM, 700 W, bench.py: 23.27 ms/frame with, 23.16-23.18 without)
 #endif
 template <bool I2F> PT_DEVICE float byteToCoord(uint w, int j, uint one) { return I2F ? float((w >> (8 * j)) & 0xFFu) : (PT_PRMT_IMM ? byteToUnitFloatImm(w, j, one) : byteToUnitFloat(w, j)); }
 
@@ -318,22 +315,6 @@ struct Traverser
                     const uint nearx = negx ? qhix : qlox, farx = negx ? qlox : qhix;
                     const uint neary = negy ? qhiy : qloy, fary = negy ? qloy : qhiy;
                     const uint nearz = negz ? qhiz : qloz, farz = negz ? qloz : qhiz;
-#if PT_FFMA2
-                    #pragma unroll
-                    for (int jj = 0; jj < 4; jj += 2)
-                    {   // children jj and jj + 1 in the two halves of each packed FMA; every lane of a pair computes exactly what the scalar form computes (fma.rn per half)
-                        const float2 t0x = __ffma2_rn(make_float2(byteToCoord<(PT_I2F_AXES > 0)>(nearx, jj, one), byteToCoord<(PT_I2F_AXES > 0)>(nearx, jj + 1, one)), make_float2(Anx, Anx), make_float2(Onx, Onx));
-                        const float2 t1x = __ffma2_rn(make_float2(byteToCoord<(PT_I2F_AXES > 0)>(farx, jj, one), byteToCoord<(PT_I2F_AXES > 0)>(farx, jj + 1, one)), make_float2(Afx, Afx), make_float2(Ofx, Ofx));
-                        const float2 t0y = __ffma2_rn(make_float2(byteToCoord<(PT_I2F_AXES > 1)>(neary, jj, one), byteToCoord<(PT_I2F_AXES > 1)>(neary, jj + 1, one)), make_float2(Any, Any), make_float2(Ony, Ony));
-                        const float2 t1y = __ffma2_rn(make_float2(byteToCoord<(PT_I2F_AXES > 1)>(fary, jj, one), byteToCoord<(PT_I2F_AXES > 1)>(fary, jj + 1, one)), make_float2(Afy, Afy), make_float2(Ofy, Ofy));
-                        const float2 t0z = __ffma2_rn(make_float2(byteToCoord<(PT_I2F_AXES > 2)>(nearz, jj, one), byteToCoord<(PT_I2F_AXES > 2)>(nearz, jj + 1, one)), make_float2(Anz, Anz), make_float2(Onz, Onz));
-                        const float2 t1z = __ffma2_rn(make_float2(byteToCoord<(PT_I2F_AXES > 2)>(farz, jj, one), byteToCoord<(PT_I2F_AXES > 2)>(farz, jj + 1, one)), make_float2(Afz, Afz), make_float2(Ofz, Ofz));
-                        if (fmaxf(fmaxf(t0x.x, t0y.x), fmaxf(t0z.x, tMin)) <= fminf(fminf(t1x.x, t1y.x), fminf(t1z.x, bestT)))
-                            hitmask |= ((childBits4 >> (8 * jj)) & 0xFFu) << ((bitIndex4 >> (8 * jj)) & 0xFFu);
-                        if (fmaxf(fmaxf(t0x.y, t0y.y), fmaxf(t0z.y, tMin)) <= fminf(fminf(t1x.y, t1y.y), fminf(t1z.y, bestT)))
-                            hitmask |= ((childBits4 >> (8 * jj + 8)) & 0xFFu) << ((bitIndex4 >> (8 * jj + 8)) & 0xFFu);
-                    }
-#else
                     #pragma unroll
                     for (int j = 0; j < 4; j++)
                     {
@@ -345,7 +326,6 @@ struct Traverser
                         if (cmin <= cmax)
                             hitmask |= ((childBits4 >> (8 * j)) & 0xFFu) << ((bitIndex4 >> (8 * j)) & 0xFFu);
                     }
-#endif
                 }
                 nodeGroup.y = (hitmask & 0xFF000000u) | imask;
                 triBits = hitmask & 0x00FFFFFFu;

@@ -18,7 +18,7 @@ class RtxptError(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile the CUDA library in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA library in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     r = subprocess.run(["make", "-C", CSRC, "-j4"], capture_output=not verbose, text=True)
     if r.returncode != 0:
         raise RtxptError("building librtxpt_b200.so failed:\n" + (r.stdout or "") + (r.stderr or ""))

@@ -14,7 +14,7 @@ def measured_peak_gbs():
     try:
         with open(p) as f: return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:  # noqa: BLE001
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def config3(args, lib, scenes, sb, S):
@@ -48,7 +48,7 @@ def config3(args, lib, scenes, sb, S):
     out.update({"image": [W, H], "spp": SPP, "warmup_frames": WARM, "frames": args.frames, "emissive_triangle_lights": int(st.lightCount) - 5368, "planes_denoised": 3,
                 "pixels_with_plane": planes, "pixels_with_feedback": float(ctl[7]) / float(px), "sampling_proxies": int(ctl[4]), "finite": bool(np.isfinite(img).all()), "mean_radiance": float(img.mean()),
                 "kernel_launches_trace": int(st.kernelLaunches), "fill_rays_last_sub_sample": rays,
-                "reblur_roofline": {"bound": "hbm (compulsory bytes; the passes are ALU-heavy, see profiles/)", "algorithmic_bytes_per_plane": int(bytes_per_plane), "planes": 3,
+                "reblur_roofline": {"bound": "hbm (compulsory bytes; the passes are ALU-heavy)", "algorithmic_bytes_per_plane": int(bytes_per_plane), "planes": 3,
                                     "achieved": 3 * bytes_per_plane / (med["denoise_ms"] * 1e-3) / 1e9, "peak": peak, "unit": "GB/s", "frac": 3 * bytes_per_plane / (med["denoise_ms"] * 1e-3) / 1e9 / peak,
                                     "peak_source": peak_src, "note": "denoise_ms covers, per plane, prepare inputs + 8 ReBLUR passes + final merge; every plane is charged the full frame although planes 1-2 cover only pixels_with_plane[1..2] of it"},
                 "timing": "update_begin_ms, frame_ms: host clock between synchronizes; trace_ms (BUILD + UpdateEnd + 4 x FILL), denoise_ms: CUDA events on the context stream; medians over the timed frames"})

@@ -1,4 +1,4 @@
-"""Workload for the `ncu --set full` capture of the wavefront kernels (profiles/r2_ncu_full_summary.json): bench.py's frame (city, 1920x1080, 4 spp, 6 bounces), 3 frames.
+"""Workload for the `ncu --set full` capture of the wavefront kernels (summarised under profiles/ by scripts/ncu_summary.py): bench.py's frame (city, 1920x1080, 4 spp, 6 bounces), 3 frames.
 One frame = k_generate + 11 x (k_trace_closest, k_shade, k_trace_shadow) + k_commit_accumulate = 35 launches; the third frame is captured:
     ncu --set full --clock-control none --import-source on -k regex:"k_generate|k_trace_|k_shade|k_commit" -s 70 -c 35 -o gpurun_out/r2_full python scripts/profile_wavefront.py"""
 import os, sys

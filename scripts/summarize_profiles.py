@@ -61,7 +61,7 @@ if os.path.exists(os.path.join(go, tag + "_bench_reference.json")):
     json.dump(last_json(os.path.join(go, tag + "_bench_reference.json")), open(os.path.join(pr, tag + "_bench_reference_n1.json"), "w"))
 km = b["roofline"]["kernel_ms_per_frame"]; tot_b = sum(km.values())
 
-md = ["# Round %s profiles (B200, sm_100a, default build)\n" % tag[1:],
+md = ["# Round %s profiles (sm_90a, default build)\n" % tag[1:],
       "Workload = `bench.py` default: %s\n" % b["config"]["workload"],
       "Bench line (`%s_bench_n1.json`): **%.0f Mrays/s, %.2f ms/frame** device-resident, e2e %.0f Mrays/s, roofline.frac %.3f (algorithmic %.0f GB/s of %.0f GB/s measured peak), "
       "ncu DRAM traffic of the traversal kernel %.2f GB/frame vs %.1f GB algorithmic.\n" % (tag, b["value"], b["ms_per_step"], b["e2e"]["value"], b["roofline"]["frac"], b["roofline"]["achieved"],

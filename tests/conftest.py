@@ -9,8 +9,8 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
-    config.addinivalue_line("markers", "gpu_unverified: GPU tests of code that has compiled but not yet run on a B200 (select with `-m gpu_unverified`); skipped without a device")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu_unverified: GPU tests of code that has compiled but not yet run on an H100 (select with `-m gpu_unverified`); skipped without a device")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -24,7 +24,7 @@ def pytest_collection_modifyitems(config, items):
     have_gpu = cuda_device_present()
     for item in items:
         if "gpu_unverified" in item.keywords and (not have_gpu or config.getoption("-m") != "gpu_unverified"):
-            item.add_marker(pytest.mark.skip(reason="not yet verified on a GPU; run with -m gpu_unverified on a B200"))
+            item.add_marker(pytest.mark.skip(reason="not yet verified on a GPU; run with -m gpu_unverified on an H100"))
 
 
 @pytest.fixture(scope="session")

@@ -301,4 +301,4 @@ def test_block_compressed_textures_render_like_their_host_decode(tmp_path, fmt):
     assert a[..., :3].mean() > 1e-3 and np.isfinite(b).all()
     rel = np.abs(a[..., :3] - b[..., :3]) / (np.abs(a[..., :3]) + 1e-2)
     if fmt == "BC7": assert np.percentile(rel, 99.9) < 2e-3 and abs(a.mean() - b.mean()) < 1e-4 * a.mean()
-    else: assert np.percentile(rel, 99) < 5e-2 and abs(a.mean() - b.mean()) < 5e-3 * a.mean()          # measured on a B200: BC1 within 2e-2, BC3 2.2e-2 (one LSB of an sRGB-encoded colour is several percent of a dark linear value)
+    else: assert np.percentile(rel, 99) < 5e-2 and abs(a.mean() - b.mean()) < 5e-3 * a.mean()          # the texture unit decodes BC1 / BC3 with its own rounding (one LSB of an sRGB-encoded colour is several percent of a dark linear value)

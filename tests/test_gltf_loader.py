@@ -169,7 +169,7 @@ def test_cpp_host_example_without_gpu(product, tmp_path):
 @pytest.mark.gpu
 def test_cpp_realtime_example_writes_a_tone_mapped_frame(product, tmp_path):
     """glTF file -> examples/realtime_gltf.cpp (NEE-AT update, stable-plane BUILD/FILL, ReBLUR, tone mapping through the C ABI only) -> PPM: the box is lit, not saturated, and the
-    image differs from a flat fill.  First run on a B200 in round 2."""
+    image differs from a flat fill."""
     import subprocess
     from rtxpt_b200 import scenes
     exe = os.path.join(os.path.dirname(product.LIB_PATH), "realtime_gltf")

@@ -1,9 +1,9 @@
-"""GPU: rtxpt_b200_bake_env_map (envbake_kernels.cu) against the oracle.  First run on a B200 in round 2 (scripts/gpu_verify_round2.sh, gpu_batch2.sh, gpu_batch3.sh); tolerances marked "measured" come from those runs.  The kernels are built with IEEE arithmetic in both libraries;
+"""GPU: rtxpt_b200_bake_env_map (envbake_kernels.cu) against the oracle.  Tolerances marked "measured" come from GPU runs of these tests.  The kernels are built with IEEE arithmetic in both libraries;
 atan2 / acos / pow / cos come from libdevice, so texels agree within a few fp16 steps rather than bit for bit - the tolerance below is a first estimate."""
 import numpy as np
 import pytest
 
-unverified = pytest.mark.gpu          # promoted in round 2 after the first green runs on a B200 (the name is kept so that the history of each test stays readable)
+unverified = pytest.mark.gpu          # promoted after the first green GPU runs (the name is kept so that the history of each test stays readable)
 
 
 @unverified

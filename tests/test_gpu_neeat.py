@@ -3,11 +3,11 @@ The baker passes are reservoir / integer bookkeeping written with single IEEE op
 already does, tests/test_neeat_port.py; here the atomics of P0, the device scan, the proxy fill and the cooperative tile sort join in).  The path-tracer side goes through libdevice
 pow / the fast-math shading, so it is held to the estimator's properties: same mean as global-only sampling, lower error, and the oracle's own feedback statistics.
 
-First run on a B200 in round 2 (scripts/gpu_verify_round2.sh, gpu_batch2.sh, gpu_batch3.sh); tolerances marked "measured" come from those runs."""
+Tolerances marked "measured" come from GPU runs of these tests."""
 import numpy as np
 import pytest
 
-unverified = pytest.mark.gpu          # promoted in round 2 after the first green runs on a B200 (the name is kept so that the history of each test stays readable)
+unverified = pytest.mark.gpu          # promoted after the first green GPU runs (the name is kept so that the history of each test stays readable)
 
 
 def _pair(product, oracle, W, H, bays=7, strict=True, bounces=2):

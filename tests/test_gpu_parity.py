@@ -95,7 +95,7 @@ def test_bsdf_against_reference_header_golden(ctx):
     live = rec[:, 33] == 255.0                  # the path always runs with LobeType::All (PathTracerBridgeDonut.hlsli:723), which is what the CUDA BSDF is specialised for; the
     rec, ref = np.ascontiguousarray(rec[live]), ref[live]      # restricted-lobe records of the fixture pin the oracle only (tests/test_oracle_golden.py)
     out = ctx.debug_bsdf(rec)
-    tol = 2e-4 if ctx.variant == "strict" else 2e-3           # fast build measured on a B200: 1.2e-3 at the 99.9th percentile of this fixture (it is denser in grazing / threshold cases than random records)
+    tol = 2e-4 if ctx.variant == "strict" else 2e-3           # the fast build is looser on this fixture (it is denser in grazing / threshold cases than random records)
     assert np.array_equal(out[:, 15], ref[:, 15])
     assert (out[:, 5] != ref[:, 5]).mean() < 1e-3
     same_lobe = (out[:, 13] == ref[:, 13]) & (out[:, 5] == ref[:, 5])
@@ -511,9 +511,9 @@ def test_config3_full_scene_realtime_neeat_reblur(product, oracle):
         assert m["planes"][1] > 0.2 and m["planes"][2] > 0.02, m                     # the decomposition has work to do in this view
         assert m["same_header"] > 0.995, (f, m)
         assert m["stable"] > 0.99, (f, m)
-        assert m["merged_close"] > 0.995, (f, m)                                   # measured on a B200: 0.9996 / 0.9995 (texture filtering, TMU vs software, changes a few paths); headers 1.0, stable radiance 0.99998
+        assert m["merged_close"] > 0.995, (f, m)                                   # texture filtering (TMU vs software) changes a few paths
         assert abs(m["mean_ratio"] - 1) < 0.02, (f, m)
-        assert min(m["reblur"].values()) > 0.995, (f, m)                           # measured: 1.0 / 1.0 / 1.0 (profiles/r2_config3_parity.log)
+        assert min(m["reblur"].values()) > 0.995, (f, m)
 
 
 @pytest.mark.gpu

@@ -3,11 +3,11 @@ C ABI: realtime path trace -> rtxpt_b200_denoiser_prepare_inputs -> rtxpt_b200_r
 its own history.  Values are fp16 images; the two sides differ by libdevice vs glibc transcendentals (exp, pow, atan, log) in weights, so the bar is agreement within a few fp16
 steps on nearly every pixel plus identical history-length bookkeeping, stated per assert.
 
-First run on a B200 in round 2 (scripts/gpu_verify_round2.sh, gpu_batch2.sh, gpu_batch3.sh); tolerances marked "measured" come from those runs."""
+Tolerances marked "measured" come from GPU runs of these tests."""
 import numpy as np
 import pytest
 
-unverified = pytest.mark.gpu          # promoted in round 2 after the first green runs on a B200 (the name is kept so that the history of each test stays readable)
+unverified = pytest.mark.gpu          # promoted after the first green GPU runs (the name is kept so that the history of each test stays readable)
 
 
 def _scene(product, strict, W, H):
@@ -63,7 +63,7 @@ def test_reblur_static_camera_matches_oracle(product, oracle, strict):
     for f in range(5):
         inputs, out = _frame(c, sb, W, H, cam, cam, consts, f, plane=0)
         od, os_, frames = rb.denoise(wv, vc, f, inputs["view_z"], inputs["normal_roughness"], inputs["diff"], inputs["spec"], motion=inputs["motion"], disocclusion_mix=inputs["disocclusion_mix"])
-        _compare(out, od, os_, frames, inputs, 0.985 if strict else 0.93, ("static", strict, f))          # fast build measured on a B200: 0.947 (specular, frame 0)
+        _compare(out, od, os_, frames, inputs, 0.985 if strict else 0.93, ("static", strict, f))
         surf = inputs["view_z"] < 1e5
         assert np.median(out["frames"][surf][:, 0]) >= min(f, 3) - 0.13                                 # history grows by one frame per frame on a static view
     rb.close(); c.close()
@@ -124,7 +124,7 @@ def test_denoise_realtime_reduces_error_and_keeps_energy(product):
         c.denoise_realtime(k, sb.make_reblur_frame(cam, cam, frame_index=f)); c.synchronize(); den = c.readback_output_color()[..., :3].astype(np.float32)
     assert np.isfinite(den).all()
     e_noisy = np.abs(np.minimum(noisy, 4) - np.minimum(ref, 4)).mean(); e_den = np.abs(np.minimum(den, 4) - np.minimum(ref, 4)).mean()
-    assert e_den < 0.6 * e_noisy, (e_den, e_noisy)                    # measured on a B200: 0.51 (the 256 spp reference still carries noise of its own: the ratio understates the gain)
+    assert e_den < 0.6 * e_noisy, (e_den, e_noisy)                    # the 256 spp reference still carries noise of its own: the ratio understates the gain
     assert abs(den.mean() - ref.mean()) < 0.1 * ref.mean(), (den.mean(), ref.mean())
     c.close()
 

@@ -1,9 +1,9 @@
-"""GPU: rtxpt_b200_update_instance_transforms (refit_kernels.cu).  First run on a B200 in round 2 (scripts/gpu_verify_round2.sh, gpu_batch2.sh, gpu_batch3.sh); tolerances marked "measured" come from those runs.  The refit re-transforms the leaf triangles with the arithmetic of the
+"""GPU: rtxpt_b200_update_instance_transforms (refit_kernels.cu).  Tolerances marked "measured" come from GPU runs of these tests.  The refit re-transforms the leaf triangles with the arithmetic of the
 scene upload, so a refitted context must trace exactly like a context (and an oracle) that was given the moved scene from the start."""
 import numpy as np
 import pytest
 
-unverified = pytest.mark.gpu          # promoted in round 2 after the first green runs on a B200 (the name is kept so that the history of each test stays readable)
+unverified = pytest.mark.gpu          # promoted after the first green GPU runs (the name is kept so that the history of each test stays readable)
 
 
 def _cornell_with(transforms):

@@ -1,9 +1,9 @@
-"""GPU: rtxpt_b200_skin_register / rtxpt_b200_skin_update (skinning_kernels.cu) + the refit.  First run on a B200 in round 2 (scripts/gpu_verify_round2.sh, gpu_batch2.sh, gpu_batch3.sh); tolerances marked "measured" come from those runs.  A context whose boxes were bent by a
+"""GPU: rtxpt_b200_skin_register / rtxpt_b200_skin_update (skinning_kernels.cu) + the refit.  Tolerances marked "measured" come from GPU runs of these tests.  A context whose boxes were bent by a
 two-joint skin must trace exactly like a fresh upload of the bent mesh (and like the oracle on it): the skin writes the same float positions a host-side blend produces."""
 import numpy as np
 import pytest
 
-unverified = pytest.mark.gpu          # promoted in round 2 after the first green runs on a B200 (the name is kept so that the history of each test stays readable)
+unverified = pytest.mark.gpu          # promoted after the first green GPU runs (the name is kept so that the history of each test stays readable)
 
 
 @unverified

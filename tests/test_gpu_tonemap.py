@@ -1,9 +1,9 @@
-"""GPU: rtxpt_b200_tone_map (tonemap_kernels.cu) against the oracle.  First run on a B200 in round 2 (scripts/gpu_verify_round2.sh, gpu_batch2.sh, gpu_batch3.sh); tolerances marked "measured" come from those runs.  log2 / pow / exp2 come from libdevice and the default library builds
+"""GPU: rtxpt_b200_tone_map (tonemap_kernels.cu) against the oracle.  Tolerances marked "measured" come from GPU runs of these tests.  log2 / pow / exp2 come from libdevice and the default library builds
 this unit with fast-math-free flags but FMA contraction, so 8-bit outputs may differ by one step on a small share of the pixels - the bound below is a first estimate."""
 import numpy as np
 import pytest
 
-unverified = pytest.mark.gpu          # promoted in round 2 after the first green runs on a B200 (the name is kept so that the history of each test stays readable)
+unverified = pytest.mark.gpu          # promoted after the first green GPU runs (the name is kept so that the history of each test stays readable)
 
 
 @unverified

@@ -1,14 +1,14 @@
 """RTXPT .material.json -> PTMaterialData (rtxpt_b200/csrc/material_json.cpp) against an independent Python restatement of PTMaterial::Read +
-FillData (Rtxpt/Materials/MaterialsBaker.cpp:160-245, :516-591, defaults MaterialsBaker.h:134-201) — on synthetic files always, and on every
-material file the reference ships (Assets/Materials, ~500 files incl. the 254 Bistro materials) when the reference tree is present.  CPU only."""
+FillData (Rtxpt/Materials/MaterialsBaker.cpp:160-245, :516-591, defaults MaterialsBaker.h:134-201) — on synthetic files and on every
+material file the reference ships (Assets/Materials, ~500 files incl. the 254 Bistro materials; stored in tests/golden/reference_materials.tar.xz).  CPU only."""
 import ctypes as C
-import glob
 import json
 import os
+import tarfile
 import numpy as np
 import pytest
 
-REF_MATERIALS = "/root/reference/Assets/Materials"
+REF_MATERIALS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_materials.tar.xz")
 
 
 def fill_data(j):
@@ -78,13 +78,12 @@ def test_material_json_synthetic(product):
         product.parse_material_json("[1, 2")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_MATERIALS), reason="reference assets not present")
 def test_material_json_on_reference_assets(product):
-    files = sorted(glob.glob(os.path.join(REF_MATERIALS, "*.material.json")) + glob.glob(os.path.join(REF_MATERIALS, "*", "*.material.json")))
-    assert len(files) > 400
+    with tarfile.open(REF_MATERIALS) as t:
+        texts = [t.extractfile(m).read().decode() for m in t.getmembers() if m.name.endswith(".material.json")]
+    assert len(texts) > 400
     emissive = transmissive = alpha = 0
-    for path in files:
-        text = open(path).read()
+    for text in texts:
         check(product, text)
         j = json.loads(text)
         emissive += any(c > 0 for c in j.get("EmissiveColor", [0])); transmissive += bool(j.get("EnableTransmission")); alpha += bool(j.get("EnableAlphaTesting"))
