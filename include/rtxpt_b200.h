@@ -431,6 +431,10 @@ typedef struct RtxptSkinDesc {
 } RtxptSkinDesc;
 RTXPT_API int rtxpt_b200_skin_register(rtxpt_ctx* ctx, const RtxptSkinDesc* desc, uint32_t* outSkinId);
 RTXPT_API int rtxpt_b200_skin_update(rtxpt_ctx* ctx, uint32_t skinId, const float* jointMatrices4x4, uint32_t numJoints, void* cudaStream);
+/* tests / debugging: what = 0 BVH nodes (80 B each), 1 leaf triangles (48 B), 2 per-triangle shade records (96 B, by global triangle id),
+ * 3 previous-position records (36 B), 4 instance table (RtxptInstanceData), 5 BVH level starts (uint32, levelCount + 1),
+ * 6 exact node boxes of the last refit (6 floats per node; empty before the first refit).  dst == NULL returns the size in *outBytes; synchronises the context's stream. */
+RTXPT_API int rtxpt_b200_debug_scene_readback(rtxpt_ctx* ctx, int what, void* dst, size_t dstBytes, size_t* outBytes);
 /* host-only inspection of the builder: the compressed BVH over a triangle soup (nodes 80 B, leaf triangles 48 B with gid = soup index, level ranges); call with NULL outputs for sizes */
 RTXPT_API int rtxpt_b200_debug_build_bvh(const float* triangleVertices, uint32_t triangleCount, void* outNodes, void* outTris, uint32_t* outLevelStart,
                                          uint32_t* outNodeCount, uint32_t* outTriCount, uint32_t* outLevelCount);

@@ -1060,6 +1060,31 @@ extern "C" RTXPT_API int rtxpt_b200_skin_update(rtxpt_ctx* c, uint32_t skinId, c
     CU(cudaGetLastError());
     return RTXPT_OK;
 }
+// tests / debugging: the scene state the refit and skinning kernels write (include/rtxpt_b200.h lists the `what` codes); dst == NULL returns the size only
+extern "C" RTXPT_API int rtxpt_b200_debug_scene_readback(rtxpt_ctx* c, int what, void* dst, size_t dstBytes, size_t* outBytes)
+{
+    if (!c || !outBytes) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (!c->haveScene) return fail(RTXPT_ERR_NO_SCENE, "no scene uploaded");
+    cudaSetDevice(c->device);
+    CU(syncContext(c));
+    const void* src = nullptr; size_t bytes = 0; bool host = false;
+    switch (what)
+    {
+    case 0: src = c->dBvhNodes.ptr; bytes = size_t(c->bvhNodeCount) * 80; break;
+    case 1: src = c->dBvhTris.ptr; bytes = size_t(c->bvhTriCount) * 48; break;
+    case 2: src = c->dTriShade.ptr; bytes = c->dTriShade.count * sizeof(uint4); break;
+    case 3: src = c->dTriPrevPos.ptr; bytes = c->prevPosTriangles * 36; break;
+    case 4: src = c->dInstances.ptr; bytes = c->hInstances.size() * sizeof(RtxptInstanceData); break;
+    case 5: src = c->bvhLevelStart.data(); bytes = c->bvhLevelStart.size() * 4; host = true; break;
+    case 6: src = c->dNodeBox.ptr; bytes = c->dNodeBox.count * 4; break;
+    default: return fail(RTXPT_ERR_INVALID_ARGUMENT, "unknown scene buffer %d", what);
+    }
+    *outBytes = bytes;
+    if (!dst || bytes == 0) return RTXPT_OK;
+    if (dstBytes < bytes) return fail(RTXPT_ERR_INVALID_ARGUMENT, "destination too small (%zu < %zu)", dstBytes, bytes);
+    if (host) memcpy(dst, src, bytes); else CU(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
+    return RTXPT_OK;
+}
 
 // ---- environment-map baking (SURVEY §8f row 3) ---------------------------------------------------------------------------------------------------------------------
 extern "C" RTXPT_API uint32_t rtxpt_b200_env_bake_mip_count(uint32_t cubeDim) { uint32_t l = 0; while ((cubeDim >> l) > 0) l++; return l; }

@@ -65,6 +65,7 @@ _SIGNATURES = {
     "rtxpt_b200_host_bake_opacity_mask": [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p],
     "rtxpt_b200_neeat_reset": [C.c_void_p],
     "rtxpt_b200_neeat_readback": [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)],
+    "rtxpt_b200_debug_scene_readback": [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)],
     "rtxpt_b200_neeat_debug_set_feedback": [C.c_void_p, C.c_void_p, C.c_void_p],
     "rtxpt_b200_denoise_spec_hit_t": [C.c_void_p, C.c_void_p],
     "rtxpt_b200_reblur_denoise": [C.c_void_p, C.c_uint32, C.POINTER(S.ReblurFrame), C.c_void_p],
@@ -359,6 +360,23 @@ class Context:
     def skin_update(self, skin_id, joint_matrices, stream=None):
         m = np.ascontiguousarray(joint_matrices, np.float32).reshape(-1, 16)
         _check(self.L.rtxpt_b200_skin_update(self.h, skin_id, m.ctypes.data, len(m), stream), self.L)
+
+    # (dtype, words per row) of rtxpt_b200_debug_scene_readback's buffers; 4 (the instance table) is returned as structs.InstanceData
+    _SCENE_RAW = {0: (np.uint32, 20), 1: (np.uint32, 12), 2: (np.uint32, 24), 3: (np.float32, 9), 5: (np.uint32, 1), 6: (np.float32, 6)}
+
+    def scene_raw(self, what):
+        """Tests / debugging: the scene state on the device (0 BVH nodes, 1 leaf triangles, 2 shade records, 3 previous positions, 4 instances, 5 level starts, 6 exact node boxes);
+        one row per node / triangle / record, level starts as a flat array."""
+        n = C.c_size_t()
+        _check(self.L.rtxpt_b200_debug_scene_readback(self.h, what, None, 0, C.byref(n)), self.L)
+        if what == 4:
+            out = (S.InstanceData * (n.value // C.sizeof(S.InstanceData)))()
+            _check(self.L.rtxpt_b200_debug_scene_readback(self.h, what, out, n.value, C.byref(n)), self.L)
+            return out
+        dtype, row = self._SCENE_RAW[what]
+        out = np.zeros(n.value // 4, dtype)
+        _check(self.L.rtxpt_b200_debug_scene_readback(self.h, what, out.ctypes.data, out.nbytes, C.byref(n)), self.L)
+        return out if row == 1 else out.reshape(-1, row)
 
     def tone_map(self, params, source=None, stream=None):
         """ToneMappingPass on the output colour (default) or the accumulation buffer; returns nothing - read the SRGBA8 result with readback_ldr()."""

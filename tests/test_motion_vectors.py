@@ -119,6 +119,13 @@ def test_gpu_motion_vectors_after_instance_update_and_skinning(product, oracle, 
     # 2. the same matrices again: nothing moved since last frame
     c.update_instance_transforms(np.stack([ident, ident, moved])); c.path_trace_realtime(True); c.synchronize(); g = c.readback_realtime()
     assert np.abs(g["motion"].astype(np.float32)[..., :2]).max() < 1e-3
+    # 2b. a rotation about an oblique axis and a mirror (det < 0) about the boxes' centre: normals go through xfVector of a matrix that flips the winding
+    from test_gpu_refit import about, rotation
+    turned = about(rotation((1.0, 2.0, -0.7), 0.35) @ np.diag([-1.0, 1.0, 1.0]), (2.77, 1.2, 2.6), (0.1, 0.0, 0.1))
+    c.update_instance_transforms(np.stack([ident, ident, turned])); c.path_trace_realtime(True); c.synchronize(); g = c.readback_realtime()
+    bm = _builder(boxes_prev=moved); bm.instances[2] = (bm.instances[2][0], turned)
+    _, _, _, o, _ = _pair(oracle, bm); r = o.render_realtime(rt); o.close()
+    mv = _compare_motion(g, r, strict); assert (np.abs(mv[..., :2]).max(-1) > 1e-2).mean() > 0.05
     # 3. skinning: the top of the short box leans 0.35 to +x; the records' old corners become the previous-position stream
     c.update_instance_transforms(np.stack([ident, ident, ident]))
     geo = b.meshes[b.instances[2][0]][0]; pos = np.asarray(geo["positions"], np.float32).reshape(-1, 3)

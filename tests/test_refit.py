@@ -106,3 +106,19 @@ def test_refit_edge_cases(product):
         n2, t2, b2 = _refit(emu, nodes, tris, rec, flat, levels)
         _check_tree(n2, t2, b2)
         assert (t2.view(np.float32).reshape(-1, 3, 4)[:, :, 1] == 2.0).all()
+        # scale 0 on every axis (how hosts hide an instance): every triangle of it collapses onto the translation.  All instances collapsed: every node is a point box
+        # with the smallest frame exponent (bvh8FrameExponent(0) = -126, stored biased as 1), zero child grid offsets and finite corners
+        point = np.float32([3.5, -2.25, 7.0])
+        collapsed = np.hstack([np.zeros((3, 3)), point[:, None]])
+        n3, t3, b3 = _refit(emu, nodes, tris, rec, [collapsed] * 2, levels)
+        _check_tree(n3, t3, b3)
+        assert (t3.view(np.float32).reshape(-1, 3, 4)[:, :, :3] == point).all()
+        assert np.isfinite(b3).all() and (b3[:, :3] == point).all() and (b3[:, 3:] == point).all()
+        assert (n3[:, 0:3].view(np.float32) == point).all()
+        assert ((n3[:, 3] & 0xFF) == 1).all() and (((n3[:, 3] >> 8) & 0xFF) == 1).all() and (((n3[:, 3] >> 16) & 0xFF) == 1).all()
+        assert (n3[:, 8:20] == 0).all()
+        assert np.array_equal(n3[:, 3] >> 24, nodes[:, 3] >> 24) and np.array_equal(n3[:, 4:8], nodes[:, 4:8])
+        # one instance collapsed inside a moving scene: the tree stays conservative and the collapsed triangles sit on the point
+        n4, t4, b4 = _refit(emu, nodes, tris, rec, [collapsed, flat[0]], levels)
+        _check_tree(n4, t4, b4)
+        assert np.isfinite(b4).all() and (t4.view(np.float32).reshape(-1, 3, 4)[inst[t4[:, 3]] == 0, :, :3] == point).all()
