@@ -694,6 +694,9 @@ RTXPT_API int rtxpt_b200_debug_bsdf(rtxpt_ctx* ctx, const float* in, uint32_t co
 /* Stateless sample generators evaluated on the device: out[i*8..] = 4 uniform + 4 low-discrepancy draws for
  * (pixelX,pixelY,vertexIndex,sampleIndex) tuples in `in` (4 u32 each). */
 RTXPT_API int rtxpt_b200_debug_rng(rtxpt_ctx* ctx, const uint32_t* in, uint32_t count, uint32_t* out);
+/* Leak checks: the number of CUDA resources (device arrays, streams, events, textures, pinned blocks) all contexts of the process hold right now.
+ * Destroying a context returns it to what it was before the context was created. */
+RTXPT_API int rtxpt_b200_debug_live_resources(uint64_t* out);
 
 #ifdef __cplusplus
 }

@@ -13,12 +13,15 @@
 #include "skinning.cuh"
 #include "lights_bake.h"
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 using namespace pt;
@@ -42,21 +45,58 @@ static int fail(int code, const char* fmt, ...)
 }
 #define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(e_ == cudaErrorMemoryAllocation ? RTXPT_ERR_OUT_OF_MEMORY : RTXPT_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); } while (0)
 
+// Every CUDA resource the library holds belongs to one of the two owner types below, so that an early return (CU) or a destroyed context frees
+// whatever was made so far.  g_liveResources counts what they hold across the process (rtxpt_b200_debug_live_resources).
+static std::atomic<uint64_t> g_liveResources{ 0 };
+
 template <typename T> struct DeviceArray
 {
     T* ptr = nullptr; size_t count = 0;
-    cudaError_t alloc(size_t n) { release(); count = n; if (n == 0) return cudaSuccess; return cudaMalloc(&ptr, n * sizeof(T)); }
+    DeviceArray() = default; DeviceArray(const DeviceArray&) = delete; DeviceArray& operator=(const DeviceArray&) = delete;
+    DeviceArray(DeviceArray&& o) noexcept : ptr(std::exchange(o.ptr, nullptr)), count(std::exchange(o.count, 0)) {}
+    DeviceArray& operator=(DeviceArray&& o) noexcept { if (this != &o) { reset(); ptr = std::exchange(o.ptr, nullptr); count = std::exchange(o.count, 0); } return *this; }
+    ~DeviceArray() { reset(); }
+    cudaError_t alloc(size_t n) { reset(); if (n == 0) return cudaSuccess; cudaError_t e = cudaMalloc(&ptr, n * sizeof(T)); if (e != cudaSuccess) { ptr = nullptr; return e; } g_liveResources++; count = n; return cudaSuccess; }
     cudaError_t upload(const T* src, size_t n, cudaStream_t s) { cudaError_t e = alloc(n); if (e != cudaSuccess || n == 0) return e; return cudaMemcpyAsync(ptr, src, n * sizeof(T), cudaMemcpyHostToDevice, s); }
-    void release() { if (ptr) cudaFree(ptr); ptr = nullptr; count = 0; }
+    cudaError_t fill(int byte, cudaStream_t s) const { return cudaMemsetAsync(ptr, byte, count * sizeof(T), s); }
+private:
+    void reset() { if (ptr) { cudaFree(ptr); g_liveResources--; } ptr = nullptr; count = 0; }
 };
 
-struct DeviceTexture { cudaMipmappedArray_t array = nullptr; cudaTextureObject_t object = 0; };
+// one stream, event, texture object, mipmapped array or pinned host block, destroyed by Destroy; reads as the raw handle
+template <typename T, auto Destroy> struct Owned
+{
+    Owned() = default; Owned(const Owned&) = delete; Owned& operator=(const Owned&) = delete;
+    Owned(Owned&& o) noexcept : h(std::exchange(o.h, T{})) {}
+    Owned& operator=(Owned&& o) noexcept { if (this != &o) { reset(); h = std::exchange(o.h, T{}); } return *this; }
+    ~Owned() { reset(); }
+    operator T() const { return h; }
+    // make(&handle, args...): a CUDA creation call; replaces what was held before
+    template <typename F, typename... A> cudaError_t create(F make, A... args) { reset(); cudaError_t e = make(&h, args...); if (e != cudaSuccess) h = T{}; else if (h) g_liveResources++; return e; }
+private:
+    T h{};
+    void reset() { if (h) { Destroy(h); g_liveResources--; } h = T{}; }
+};
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+
+// members are destroyed in reverse order: the texture object before its array
+struct DeviceTexture { Owned<cudaMipmappedArray_t, cudaFreeMipmappedArray> array; Owned<cudaTextureObject_t, cudaDestroyTextureObject> object; };
 
 struct rtxpt_ctx
 {
     RtxptConfig cfg{};
     int device = 0;
-    cudaStream_t stream = nullptr;
+    // streams and events come before the buffers, so that they outlive them when the context is destroyed
+    Stream stream;
+    // pipeline lanes: the sub-samples of one launch are split into independent wavefronts, each on its own pair of streams, so that the latency-bound tail of every
+    // persistent kernel of one lane (its last, longest rays) is filled by the CTAs of the other lanes.  Lane 0's first stream is the caller's (its `s` stays empty).
+    static const int kMaxLanes = 8;
+    struct Lane { Stream s, s2; Event evShadeDone, evShadowDone, evCommitted; } lanes[kMaxLanes];
+    Event evFork, evStart, evStop;
+    Event evDnStart, evDnStop;          // around the last rtxpt_b200_denoise_realtime
+    std::vector<Event> evPool;          // RTXPT_CFG_TIME_KERNELS: (begin,end) pairs per kernel
+    Event evCallerJoin;                 // joins lastCallerStream into `stream` (joinCallerStream)
     GridConfig grid;
     int maxSmemOptin = 0;
     // scene
@@ -64,15 +104,10 @@ struct rtxpt_ctx
     size_t l2PersistBytes = 0, l2WindowMax = 0;
     // measurement knobs, read from the environment once at creation (RTXPT_* variables; the defaults measured fastest on an H100 SXM at a 400 W power limit, bench.py workload: see the launch configuration)
     struct Tuning { int refillThreshold = 24, waitFlushLanes = 8, traceCtas = 4, shadeCtas = 4, smemNodes = 0, lanes = 1, shadowLpt = 1; } tune; float sceneDiagonal = 0;
-    cudaStream_t stream2 = nullptr; cudaEvent_t evShadeDone = nullptr, evShadowDone = nullptr; bool overlapShadow = true;
-    // pipeline lanes: the sub-samples of one launch are split into independent wavefronts, each on its own pair of streams, so that the latency-bound tail of every
-    // persistent kernel of one lane (its last, longest rays) is filled by the CTAs of the other lanes.  Lane 0 is (caller stream, stream2).
-    static const int kMaxLanes = 8;
-    struct Lane { cudaStream_t s = nullptr, s2 = nullptr; cudaEvent_t evShadeDone = nullptr, evShadowDone = nullptr, evCommitted = nullptr; } lanes[kMaxLanes];
-    cudaEvent_t evFork = nullptr; uint32_t lastLanes = 1, lastSubSamplesPerLaunch = 1;
+    bool overlapShadow = true; uint32_t lastLanes = 1, lastSubSamplesPerLaunch = 1;
     DeviceArray<RtxptInstanceData> dInstances; DeviceArray<RtxptGeometryData> dGeometries; DeviceArray<RtxptSubInstanceData> dSubInstances;
     DeviceArray<RtxptMaterialData> dMaterials; DeviceArray<uint8_t> dSubInstanceClass;
-    std::vector<uint8_t*> bufferAllocs; DeviceArray<const uint8_t*> dBufferTable;
+    std::vector<DeviceArray<uint8_t>> bufferAllocs; DeviceArray<const uint8_t*> dBufferTable;
     std::vector<DeviceTexture> textures; DeviceArray<cudaTextureObject_t> dTextureTable;
     DeviceTexture envCube; uint32_t envFaceSize = 0, envMipLevels = 0;
     DeviceArray<uint4> dBvhNodes; DeviceArray<float4> dBvhTris; DeviceArray<uint4> dTriInfo, dTriShade, dOpacityMasks;
@@ -84,7 +119,7 @@ struct rtxpt_ctx
     std::vector<uint32_t> hPrevPosBase; DeviceArray<uint32_t> dPrevPosBase; DeviceArray<float> dTriPrevPos; size_t prevPosTriangles = 0;
     struct Skin { uint32_t numVertices = 0, numTriangles = 0, firstGid = 0, flags = 0, numJoints = 0, maxJoint = 0, prevPosFirst = 0; const uint32_t* dIndices = nullptr;
                   DeviceArray<float> positions, weights, outPositions, jointMatrices; DeviceArray<uint32_t> normals, tangents, outNormals, outTangents; DeviceArray<unsigned short> jointIndices; };
-    std::vector<Skin*> skins;
+    std::vector<std::unique_ptr<Skin>> skins;
     uint32_t bvhNodeCount = 0, bvhTriCount = 0; float bvhBuildSeconds = 0;
     std::vector<RtxptSubInstanceData> hSubInstances; uint32_t materialCount = 0;
     LightBakeState lightState;
@@ -111,8 +146,6 @@ struct rtxpt_ctx
     {
         DeviceArray<float> prevViewZ; DeviceArray<uint32_t> prevNormalRoughness; DeviceArray<uint16_t> prevInternalData, diffFast, specFast, tracking[2], diffLuma[2], specLuma[2];
         DeviceArray<uint2> diffHistory, specHistory; bool valid = false; uint32_t pingPong = 0;
-        void release() { prevViewZ.release(); prevNormalRoughness.release(); prevInternalData.release(); diffFast.release(); specFast.release(); diffHistory.release(); specHistory.release();
-                         for (int i = 0; i < 2; i++) { tracking[i].release(); diffLuma[i].release(); specLuma[i].release(); } valid = false; }
     } reblur[RTXPT_STABLE_PLANE_COUNT];
     DeviceArray<uint8_t> rbTiles; DeviceArray<uint2> rbTmp1Diff, rbTmp1Spec, rbTmp2Diff, rbTmp2Spec, rbOutDiff, rbOutSpec; DeviceArray<uint16_t> rbTrackingT, rbDiffFastT, rbSpecFastT; DeviceArray<uchar2> rbData1; DeviceArray<uint32_t> rbData2;
     uint32_t reblurWidth = 0, reblurHeight = 0;
@@ -125,20 +158,16 @@ struct rtxpt_ctx
         DeviceArray<float> weights[2], weightGroupSums, weightsSum; uint32_t weightPingPong = 0;      // boosted weights: this frame / last frame
         // dynamic light lists: the list last frame's feedback was indexed by, and this frame's past <-> current index tables (NULL pointers in params while the list stands still)
         LightListSnapshot snap; uint64_t snapVersion = 0; bool remapActive = false; uint32_t lightCapacity = 0; DeviceArray<uint32_t> pastToCurrent, currentToPast; std::vector<uint32_t> hPastToCurrent, hCurrentToPast;
-        void release() { fbWeight.release(); scratchWeight.release(); blendedWeight.release(); historyDepth.release(); lightWeights.release(); fbCandidate.release(); scratchCandidate.release();
-                         blendedCandidate.release(); local.release(); counters.release(); proxyCounters.release(); proxyOffsets.release(); proxyIndices.release(); samplingProxyCount.release();
-                         scanBlockSums.release(); rrFix.release(); shadowFeedback.release(); weights[0].release(); weights[1].release(); weightGroupSums.release(); weightsSum.release(); pastToCurrent.release(); currentToPast.release(); snap = LightListSnapshot(); remapActive = false; lightCapacity = 0; allocated = false; frameBegun = false; frameEnded = false; }
     } na;
     DeviceArray<double> tmPartials; DeviceArray<float> tmAvgLuminance; DeviceArray<uint32_t> ldrColor; bool toneMapped = false;      // tone mapping (tonemap.cuh)
-    cudaEvent_t evDnStart = nullptr, evDnStop = nullptr; bool denoiseTimed = false;       // around the last rtxpt_b200_denoise_realtime
+    bool denoiseTimed = false;
     // stats
-    uint32_t* hCounters = nullptr;          // pinned
-    cudaEvent_t evStart = nullptr, evStop = nullptr;
-    std::vector<cudaEvent_t> evPool; std::vector<int> evKind; size_t evUsed = 0;     // RTXPT_CFG_TIME_KERNELS: (begin,end) pairs per kernel
+    Owned<uint32_t*, cudaFreeHost> hCounters;          // pinned
+    std::vector<int> evKind; size_t evUsed = 0;
     uint32_t lastIterations = 0, lastSubSamples = 0; uint64_t lastLaunches = 0;
     bool statsPending = false;
     // the caller's stream that last received work through this context (null: everything went to `stream`); host reads join it first
-    cudaStream_t lastCallerStream = nullptr; cudaEvent_t evCallerJoin = nullptr;
+    cudaStream_t lastCallerStream = nullptr;
 };
 
 static const uint32_t kCounterWords = (kMaxWavefrontIterations + 2) * kCountersPerIter;
@@ -156,7 +185,7 @@ static cudaError_t joinCallerStream(rtxpt_ctx* c)
 {
     if (!c->lastCallerStream) return cudaSuccess;
     cudaError_t e;
-    if (!c->evCallerJoin && (e = cudaEventCreateWithFlags(&c->evCallerJoin, cudaEventDisableTiming)) != cudaSuccess) return e;
+    if (!c->evCallerJoin && (e = c->evCallerJoin.create(cudaEventCreateWithFlags, cudaEventDisableTiming)) != cudaSuccess) return e;
     if ((e = cudaEventRecord(c->evCallerJoin, c->lastCallerStream)) != cudaSuccess) return e;
     return cudaStreamWaitEvent(c->stream, c->evCallerJoin, 0);
 }
@@ -166,15 +195,8 @@ extern "C" RTXPT_API const char* rtxpt_b200_last_error(void) { return g_lastErro
 
 static void releaseScene(rtxpt_ctx* c)
 {
-    for (rtxpt_ctx::Skin* sk : c->skins) { sk->positions.release(); sk->weights.release(); sk->outPositions.release(); sk->jointMatrices.release(); sk->normals.release(); sk->tangents.release(); sk->outNormals.release(); sk->outTangents.release(); sk->jointIndices.release(); delete sk; }
-    c->skins.clear();
-    for (uint8_t* p : c->bufferAllocs) cudaFree(p);
-    c->bufferAllocs.clear();
-    for (DeviceTexture& t : c->textures) { if (t.object) cudaDestroyTextureObject(t.object); if (t.array) cudaFreeMipmappedArray(t.array); }
-    c->textures.clear();
-    if (c->envCube.object) cudaDestroyTextureObject(c->envCube.object);
-    if (c->envCube.array) cudaFreeMipmappedArray(c->envCube.array);
-    c->envCube = DeviceTexture();
+    c->skins.clear(); c->bufferAllocs.clear(); c->textures.clear();
+    std::exchange(c->envCube, DeviceTexture());        // the old cube is destroyed at the end of the statement, its texture object before its array
     c->haveScene = false;
 }
 
@@ -184,34 +206,37 @@ extern "C" RTXPT_API int rtxpt_b200_create(const RtxptConfig* config, rtxpt_ctx*
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n == 0) return fail(RTXPT_ERR_NO_DEVICE, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
-    rtxpt_ctx* c = new rtxpt_ctx();
+    std::unique_ptr<rtxpt_ctx> c(new rtxpt_ctx());
     c->cfg = *config;
     if (c->cfg.maxSubSamplesPerLaunch == 0) c->cfg.maxSubSamplesPerLaunch = 1;
     if (c->cfg.tileWorld == 0) { c->cfg.tileWorld = 1; c->cfg.tileRank = 0; }
     if (c->cfg.tileSize == 0) c->cfg.tileSize = 64;
-    if (c->cfg.tileRank >= c->cfg.tileWorld || (c->cfg.tileSize & (c->cfg.tileSize - 1)) != 0) { delete c; return fail(RTXPT_ERR_INVALID_ARGUMENT, "bad tile partition"); }
-    if (config->deviceOrdinal >= 0) { if (cudaSetDevice(config->deviceOrdinal) != cudaSuccess) { delete c; return fail(RTXPT_ERR_NO_DEVICE, "cudaSetDevice(%d) failed", config->deviceOrdinal); } }
+    if (c->cfg.tileRank >= c->cfg.tileWorld || (c->cfg.tileSize & (c->cfg.tileSize - 1)) != 0) return fail(RTXPT_ERR_INVALID_ARGUMENT, "bad tile partition");
+    if (config->deviceOrdinal >= 0) { if (cudaSetDevice(config->deviceOrdinal) != cudaSuccess) return fail(RTXPT_ERR_NO_DEVICE, "cudaSetDevice(%d) failed", config->deviceOrdinal); }
     cudaGetDevice(&c->device);
     cudaDeviceProp prop; cudaGetDeviceProperties(&prop, c->device);
     c->grid.smCount = prop.multiProcessorCount;
     c->maxSmemOptin = int(prop.sharedMemPerBlockOptin);
-    if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return fail(RTXPT_ERR_CUDA, "stream creation failed"); }
-    cudaEventCreate(&c->evStart); cudaEventCreate(&c->evStop);
-    cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking);
-    cudaEventCreateWithFlags(&c->evShadeDone, cudaEventDisableTiming); cudaEventCreateWithFlags(&c->evShadowDone, cudaEventDisableTiming);
+    CU(c->stream.create(cudaStreamCreateWithFlags, cudaStreamNonBlocking));
+    CU(c->evStart.create(cudaEventCreateWithFlags, cudaEventDefault)); CU(c->evStop.create(cudaEventCreateWithFlags, cudaEventDefault));
     { const char* e = getenv("RTXPT_OVERLAP_SHADOW"); if (e) c->overlapShadow = atoi(e) != 0; }
     auto envInt = [](const char* name, int def, int lo, int hi) { const char* e = getenv(name); return e ? std::min(hi, std::max(lo, atoi(e))) : def; };
     c->tune.refillThreshold = envInt("RTXPT_REFILL_THRESHOLD", 24, 1, 32); c->tune.waitFlushLanes = envInt("RTXPT_WAIT_FLUSH", 8, 1, 33);
     c->tune.traceCtas = envInt("RTXPT_TRACE_CTAS", 4, 2, 4); c->tune.shadeCtas = envInt("RTXPT_SHADE_CTAS", 4, 3, 5); c->tune.smemNodes = envInt("RTXPT_SMEM_NODES", 0, 0, 1 << 20);
     c->tune.shadowLpt = envInt("RTXPT_SHADOW_LPT", 1, 0, 1);
     c->tune.lanes = envInt("RTXPT_LANES", 1, 1, rtxpt_ctx::kMaxLanes);          // H100 (400 W), bench.py, ms/frame: 1 lane 25.4-25.5, 2 lanes 25.8 (one GPU has enough rays per wavefront; lanes are for small per-rank tile sets)
-    cudaEventCreateWithFlags(&c->evFork, cudaEventDisableTiming);
-    for (int l = 1; l < rtxpt_ctx::kMaxLanes; l++) { cudaStreamCreateWithFlags(&c->lanes[l].s, cudaStreamNonBlocking); cudaStreamCreateWithFlags(&c->lanes[l].s2, cudaStreamNonBlocking); }
-    for (int l = 0; l < rtxpt_ctx::kMaxLanes; l++) { cudaEventCreateWithFlags(&c->lanes[l].evShadeDone, cudaEventDisableTiming); cudaEventCreateWithFlags(&c->lanes[l].evShadowDone, cudaEventDisableTiming); cudaEventCreateWithFlags(&c->lanes[l].evCommitted, cudaEventDisableTiming); }
-    cudaMallocHost(&c->hCounters, kCounterWords * rtxpt_ctx::kMaxLanes * sizeof(uint32_t));
+    CU(c->evFork.create(cudaEventCreateWithFlags, cudaEventDisableTiming));
+    for (int l = 0; l < rtxpt_ctx::kMaxLanes; l++)
+    {
+        rtxpt_ctx::Lane& L = c->lanes[l];
+        if (l > 0) CU(L.s.create(cudaStreamCreateWithFlags, cudaStreamNonBlocking));
+        CU(L.s2.create(cudaStreamCreateWithFlags, cudaStreamNonBlocking));
+        CU(L.evShadeDone.create(cudaEventCreateWithFlags, cudaEventDisableTiming)); CU(L.evShadowDone.create(cudaEventCreateWithFlags, cudaEventDisableTiming)); CU(L.evCommitted.create(cudaEventCreateWithFlags, cudaEventDisableTiming));
+    }
+    CU(c->hCounters.create(cudaHostAlloc<uint32_t>, kCounterWords * rtxpt_ctx::kMaxLanes * sizeof(uint32_t), cudaHostAllocDefault));
     memset(c->hCounters, 0, kCounterWords * rtxpt_ctx::kMaxLanes * sizeof(uint32_t));
     e = configureKernels(c->maxSmemOptin);
-    if (e != cudaSuccess) { delete c; return fail(RTXPT_ERR_CUDA, "kernel configuration failed: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(RTXPT_ERR_CUDA, "kernel configuration failed: %s", cudaGetErrorString(e));
     {   // L2 persistence carve-out for the BVH nodes (off unless RTXPT_L2_PERSIST_MB is set; see DESIGN.md for the measurement)
         const char* e = getenv("RTXPT_L2_PERSIST_MB"); int maxPersist = 0, maxWindow = 0;
         cudaDeviceGetAttribute(&maxPersist, cudaDevAttrMaxPersistingL2CacheSize, c->device); cudaDeviceGetAttribute(&maxWindow, cudaDevAttrMaxAccessPolicyWindowSize, c->device);
@@ -222,8 +247,8 @@ extern "C" RTXPT_API int rtxpt_b200_create(const RtxptConfig* config, rtxpt_ctx*
         }
     }
     launchInitTables(c->stream);
-    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) { delete c; return fail(RTXPT_ERR_CUDA, "table initialisation failed: %s", cudaGetErrorString(e)); }
-    *outCtx = c;
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return fail(RTXPT_ERR_CUDA, "table initialisation failed: %s", cudaGetErrorString(e));
+    *outCtx = c.release();
     return RTXPT_OK;
 }
 
@@ -232,37 +257,6 @@ extern "C" RTXPT_API int rtxpt_b200_destroy(rtxpt_ctx* c)
     if (!c) return RTXPT_OK;
     cudaSetDevice(c->device);
     syncContext(c);
-    releaseScene(c);
-    c->dInstances.release(); c->dGeometries.release(); c->dSubInstances.release(); c->dMaterials.release(); c->dSubInstanceClass.release();
-    c->dBufferTable.release(); c->dTextureTable.release(); c->dBvhNodes.release(); c->dBvhTris.release(); c->dTriInfo.release(); c->dTriShade.release(); c->dNodeBox.release(); c->dPrevPosBase.release(); c->dTriPrevPos.release();
-    c->dLightsEx.release(); c->dLights.release(); c->dProxyCounters.release(); c->dProxyIndices.release(); c->dEnvLookup.release();
-    c->s0.release(); c->s1.release(); c->s2.release(); c->s3.release(); c->s4.release(); c->hits.release();
-    c->rayQueue[0].release(); c->rayQueue[1].release(); c->shadeQueue.release();
-    c->shadowOriginTMax.release(); c->shadowDirPath.release(); c->shadowRadiance.release(); c->counters.release(); c->pixelOfSlot.release(); c->allPixelTable.release();
-    c->outputColor.release(); c->accumulated.release(); c->depth.release(); c->motionVectors.release(); c->throughput.release();
-    c->stablePlanes.release(); c->stablePlanesHeader.release(); c->stableRadiance.release(); c->specularHitT.release();
-    c->dnScratchFloat.release(); c->dnViewZ.release(); c->dnMotion.release(); c->dnDiff.release(); c->dnSpec.release(); c->dnNormalRoughness.release(); c->dnDisocclusionMix.release(); c->dnHistoryClampRelax.release();
-    for (auto& h : c->reblur) h.release();
-    c->na.release(); c->tmPartials.release(); c->tmAvgLuminance.release(); c->ldrColor.release();
-    c->rbTiles.release(); c->rbTmp1Diff.release(); c->rbTmp1Spec.release(); c->rbTmp2Diff.release(); c->rbTmp2Spec.release(); c->rbOutDiff.release(); c->rbOutSpec.release();
-    c->rbTrackingT.release(); c->rbDiffFastT.release(); c->rbSpecFastT.release(); c->rbData1.release(); c->rbData2.release();
-    for (cudaEvent_t ev : c->evPool) cudaEventDestroy(ev);
-    if (c->evCallerJoin) cudaEventDestroy(c->evCallerJoin);
-    if (c->evStart) cudaEventDestroy(c->evStart);
-    if (c->evStop) cudaEventDestroy(c->evStop);
-    if (c->hCounters) cudaFreeHost(c->hCounters);
-    if (c->evDnStart) cudaEventDestroy(c->evDnStart);
-    if (c->evDnStop) cudaEventDestroy(c->evDnStop);
-    if (c->evFork) cudaEventDestroy(c->evFork);
-    for (int l = 0; l < rtxpt_ctx::kMaxLanes; l++)
-    {
-        if (c->lanes[l].evShadeDone) cudaEventDestroy(c->lanes[l].evShadeDone); if (c->lanes[l].evShadowDone) cudaEventDestroy(c->lanes[l].evShadowDone); if (c->lanes[l].evCommitted) cudaEventDestroy(c->lanes[l].evCommitted);
-        if (l > 0 && c->lanes[l].s) cudaStreamDestroy(c->lanes[l].s); if (l > 0 && c->lanes[l].s2) cudaStreamDestroy(c->lanes[l].s2);
-    }
-    if (c->evShadeDone) cudaEventDestroy(c->evShadeDone);
-    if (c->evShadowDone) cudaEventDestroy(c->evShadowDone);
-    if (c->stream2) cudaStreamDestroy(c->stream2);
-    if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
     return RTXPT_OK;
 }
@@ -291,7 +285,7 @@ static int createTexture2D(const RtxptTextureDesc& d, DeviceTexture& out)
         default:                     fmt = cudaCreateChannelDesc<cudaChannelFormatKindUnsignedBlockCompressed7SRGB>(); blockBytes = 16; break;
         }
     }
-    CU(cudaMallocMipmappedArray(&out.array, &fmt, make_cudaExtent(d.width, d.height, 0), d.mipLevels));
+    CU(out.array.create(cudaMallocMipmappedArray, &fmt, make_cudaExtent(d.width, d.height, 0), d.mipLevels, 0u));
     const size_t texel = isFloat ? 16 : 4;
     for (uint32_t m = 0; m < d.mipLevels; m++)
     {
@@ -309,7 +303,7 @@ static int createTexture2D(const RtxptTextureDesc& d, DeviceTexture& out)
     td.sRGB = (d.format == RTXPT_FORMAT_RGBA8_SRGB || d.format == RTXPT_FORMAT_BC1_SRGB || d.format == RTXPT_FORMAT_BC2_SRGB || d.format == RTXPT_FORMAT_BC3_SRGB || d.format == RTXPT_FORMAT_BC7_SRGB) ? 1 : 0;
     // (measured with scripts/probes/bc_probe.cu: the *SRGB block-compressed kinds are refused without td.sRGB, every block-compressed kind is refused with cudaReadModeElementType)
     td.normalizedCoords = 1; td.maxAnisotropy = 1; td.minMipmapLevelClamp = 0; td.maxMipmapLevelClamp = float(d.mipLevels - 1);
-    CU(cudaCreateTextureObject(&out.object, &res, &td, nullptr));
+    CU(out.object.create(cudaCreateTextureObject, &res, &td, nullptr));
     return RTXPT_OK;
 }
 
@@ -317,7 +311,7 @@ static int createEnvCube(const RtxptEnvCubeDesc& d, DeviceTexture& out)
 {
     if (d.mipLevels == 0 || d.mipLevels > RTXPT_MAX_MIPS) return fail(RTXPT_ERR_INVALID_ARGUMENT, "bad env cube description");
     cudaChannelFormatDesc fmt = cudaCreateChannelDesc<float4>();
-    CU(cudaMallocMipmappedArray(&out.array, &fmt, make_cudaExtent(d.faceSize, d.faceSize, 6), d.mipLevels, cudaArrayLayered));
+    CU(out.array.create(cudaMallocMipmappedArray, &fmt, make_cudaExtent(d.faceSize, d.faceSize, 6), d.mipLevels, cudaArrayLayered));
     for (uint32_t m = 0; m < d.mipLevels; m++)
     {
         cudaArray_t level; CU(cudaGetMipmappedArrayLevel(&level, out.array, m));
@@ -336,7 +330,7 @@ static int createEnvCube(const RtxptEnvCubeDesc& d, DeviceTexture& out)
     td.addressMode[0] = td.addressMode[1] = cudaAddressModeClamp; td.addressMode[2] = cudaAddressModeClamp;
     td.filterMode = cudaFilterModeLinear; td.mipmapFilterMode = cudaFilterModePoint; td.readMode = cudaReadModeElementType;
     td.normalizedCoords = 1; td.maxAnisotropy = 1; td.maxMipmapLevelClamp = float(d.mipLevels - 1);
-    CU(cudaCreateTextureObject(&out.object, &res, &td, nullptr));
+    CU(out.object.create(cudaCreateTextureObject, &res, &td, nullptr));
     return RTXPT_OK;
 }
 
@@ -471,22 +465,18 @@ extern "C" RTXPT_API int rtxpt_b200_upload_scene(rtxpt_ctx* c, const RtxptSceneD
     prevPosBase.resize(std::max<size_t>(prevPosBase.size(), sc->subInstanceCount), 0xFFFFFFFFu);
     c->hPrevPosBase = prevPosBase; c->prevPosTriangles = triPrevPos.size() / 9;
     CU(c->dPrevPosBase.upload(prevPosBase.data(), prevPosBase.size(), s));
-    if (!triPrevPos.empty()) CU(c->dTriPrevPos.upload(triPrevPos.data(), triPrevPos.size(), s)); else c->dTriPrevPos.release();
-    if (!masks.empty()) CU(c->dOpacityMasks.upload(masks.data(), masks.size(), s)); else c->dOpacityMasks.release();
+    CU(c->dTriPrevPos.upload(triPrevPos.data(), triPrevPos.size(), s));
+    CU(c->dOpacityMasks.upload(masks.data(), masks.size(), s));
     CU(c->dInstances.upload(sc->instances, sc->instanceCount, s));
-    c->hInstances.assign(sc->instances, sc->instances + sc->instanceCount); c->bvhLevelStart = bvh.levelStart; c->dNodeBox.release();
+    c->hInstances.assign(sc->instances, sc->instances + sc->instanceCount); c->bvhLevelStart = bvh.levelStart; c->dNodeBox = {};
     c->hGeometries.assign(sc->geometries, sc->geometries + sc->geometryCount); c->firstGidOfSubInstance = firstGid; c->maxVertexOfSubInstance = maxVertex;
     CU(c->dGeometries.upload(sc->geometries, sc->geometryCount, s));
     CU(c->dMaterials.upload(sc->materials, sc->materialCount, s));
     c->materialCount = sc->materialCount;
     // bindless buffers
     std::vector<const uint8_t*> table(sc->bufferCount, nullptr);
-    for (uint32_t i = 0; i < sc->bufferCount; i++)
-    {
-        uint8_t* p = nullptr;
-        if (sc->buffers[i].sizeBytes) { CU(cudaMalloc(&p, sc->buffers[i].sizeBytes)); c->bufferAllocs.push_back(p); CU(cudaMemcpyAsync(p, sc->buffers[i].data, sc->buffers[i].sizeBytes, cudaMemcpyHostToDevice, s)); }
-        table[i] = p;
-    }
+    c->bufferAllocs.resize(sc->bufferCount);
+    for (uint32_t i = 0; i < sc->bufferCount; i++) { CU(c->bufferAllocs[i].upload(static_cast<const uint8_t*>(sc->buffers[i].data), sc->buffers[i].sizeBytes, s)); table[i] = c->bufferAllocs[i].ptr; }
     CU(c->dBufferTable.upload(table.data(), table.size(), s));
     c->hBufferTable = table;
     // bindless textures
@@ -576,8 +566,7 @@ static int ensureTargets(rtxpt_ctx* c, uint32_t W, uint32_t H)
     }
     const size_t P = size_t(W) * H;
     CU(c->outputColor.alloc(P)); CU(c->accumulated.alloc(P)); CU(c->depth.alloc(P)); CU(c->motionVectors.alloc(P)); CU(c->throughput.alloc(P));
-    CU(cudaMemsetAsync(c->motionVectors.ptr, 0, P * sizeof(uint2), c->stream)); CU(cudaMemsetAsync(c->throughput.ptr, 0, P * sizeof(uint32_t), c->stream));
-    CU(cudaMemsetAsync(c->outputColor.ptr, 0, P * sizeof(uint2), c->stream)); CU(cudaMemsetAsync(c->accumulated.ptr, 0, P * sizeof(float4), c->stream)); CU(cudaMemsetAsync(c->depth.ptr, 0, P * sizeof(float), c->stream));
+    CU(c->motionVectors.fill(0, c->stream)); CU(c->throughput.fill(0, c->stream)); CU(c->outputColor.fill(0, c->stream)); CU(c->accumulated.fill(0, c->stream)); CU(c->depth.fill(0, c->stream));
     const size_t cap = size_t(c->pixelCount) * c->cfg.maxSubSamplesPerLaunch;
     if (cap >= 0x7FFFFFFFull) return fail(RTXPT_ERR_UNSUPPORTED, "too many path slots");
     c->capacity = uint32_t(std::max<size_t>(cap, 1));
@@ -665,7 +654,7 @@ struct KernelTimer
     void begin(int kind)
     {
         if (!on) return;
-        while (c->evPool.size() < c->evUsed + 2) { cudaEvent_t e; cudaEventCreate(&e); c->evPool.push_back(e); }
+        while (c->evPool.size() < c->evUsed + 2) { c->evPool.emplace_back(); c->evPool.back().create(cudaEventCreateWithFlags, cudaEventDefault); }
         c->evKind.resize(c->evPool.size() / 2 + 1); c->evKind[c->evUsed / 2] = kind;
         cudaEventRecord(c->evPool[c->evUsed], s);
     }
@@ -723,7 +712,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
         {
             const uint32_t firstSub = (l * n) / lanes, count = ((l + 1) * n) / lanes - firstSub;
             rtxpt_ctx::Lane& L = c->lanes[l];
-            cudaStream_t ls = l == 0 ? s : L.s, ls2 = l == 0 ? c->stream2 : L.s2;
+            cudaStream_t ls = l == 0 ? s : L.s, ls2 = L.s2;
             if (l > 0) CU(cudaStreamWaitEvent(ls, c->evFork, 0));
             LaunchParams q = p;
             {   // the lane's slice of every per-path array: slots are lane-relative, pixel = slot mod pixelCount as before
@@ -792,8 +781,7 @@ extern "C" RTXPT_API int rtxpt_b200_set_realtime(rtxpt_ctx* c, const RtxptRealti
         CU(syncContext(c));
         const size_t P = size_t(W) * H, planeStride = rtxpt_b200_generic_ts_plane_stride(W, H);
         CU(c->stablePlanes.alloc(planeStride * RTXPT_STABLE_PLANE_COUNT)); CU(c->stablePlanesHeader.alloc(P * 4)); CU(c->stableRadiance.alloc(P)); CU(c->specularHitT.alloc(P));
-        CU(cudaMemsetAsync(c->stablePlanes.ptr, 0, planeStride * RTXPT_STABLE_PLANE_COUNT * sizeof(RtxptStablePlane), c->stream));
-        CU(cudaMemsetAsync(c->stablePlanesHeader.ptr, 0xFF, P * 16, c->stream)); CU(cudaMemsetAsync(c->stableRadiance.ptr, 0, P * 8, c->stream)); CU(cudaMemsetAsync(c->specularHitT.ptr, 0, P * 4, c->stream));
+        CU(c->stablePlanes.fill(0, c->stream)); CU(c->stablePlanesHeader.fill(0xFF, c->stream)); CU(c->stableRadiance.fill(0, c->stream)); CU(c->specularHitT.fill(0, c->stream));
         c->realtimeWidth = W; c->realtimeHeight = H;
     }
     c->realtime = *rt; c->haveRealtime = true;
@@ -902,8 +890,7 @@ extern "C" RTXPT_API int rtxpt_b200_denoiser_prepare_inputs(rtxpt_ctx* c, uint32
         CU(syncContext(c));
         const size_t P = size_t(c->tableWidth) * c->tableHeight;
         CU(c->dnViewZ.alloc(P)); CU(c->dnMotion.alloc(P)); CU(c->dnDiff.alloc(P)); CU(c->dnSpec.alloc(P)); CU(c->dnNormalRoughness.alloc(P)); CU(c->dnDisocclusionMix.alloc(P)); CU(c->dnHistoryClampRelax.alloc(P));
-        CU(cudaMemsetAsync(c->dnViewZ.ptr, 0, P * 4, s)); CU(cudaMemsetAsync(c->dnMotion.ptr, 0, P * 8, s)); CU(cudaMemsetAsync(c->dnDiff.ptr, 0, P * 8, s)); CU(cudaMemsetAsync(c->dnSpec.ptr, 0, P * 8, s));
-        CU(cudaMemsetAsync(c->dnNormalRoughness.ptr, 0, P * 4, s)); CU(cudaMemsetAsync(c->dnDisocclusionMix.ptr, 0, P, s)); CU(cudaMemsetAsync(c->dnHistoryClampRelax.ptr, 0, P, s));
+        CU(c->dnViewZ.fill(0, s)); CU(c->dnMotion.fill(0, s)); CU(c->dnDiff.fill(0, s)); CU(c->dnSpec.fill(0, s)); CU(c->dnNormalRoughness.fill(0, s)); CU(c->dnDisocclusionMix.fill(0, s)); CU(c->dnHistoryClampRelax.fill(0, s));
         c->denoiserWidth = c->tableWidth; c->denoiserHeight = c->tableHeight;
     }
     LaunchParams p; fillParams(c, p); fillRealtimeParams(c, p);
@@ -1004,40 +991,33 @@ extern "C" RTXPT_API int rtxpt_b200_skin_register(rtxpt_ctx* c, const RtxptSkinD
     if (g.numIndices && maxIndex >= d->numVertices) return fail(RTXPT_ERR_INVALID_ARGUMENT, "geometry indexes vertex %u, bind pose has %u vertices", maxIndex, d->numVertices);
     cudaSetDevice(c->device);
     cudaStream_t s = c->stream;
-    rtxpt_ctx::Skin* sk = new rtxpt_ctx::Skin();
+    auto sk = std::make_unique<rtxpt_ctx::Skin>();
     sk->maxJoint = maxJoint;
     sk->numVertices = d->numVertices; sk->numTriangles = g.numIndices / 3; sk->firstGid = c->firstGidOfSubInstance[inst.firstGeometryInstanceIndex + d->geometryIndexInInstance];
     sk->flags = (d->normals ? 2u : 0u) | (d->tangents ? 4u : 0u);
     sk->dIndices = reinterpret_cast<const uint32_t*>(c->hBufferTable[g.indexBufferIndex] + g.indexOffset);
-    cudaError_t e = sk->positions.upload(d->positions, size_t(d->numVertices) * 3, s);
-    if (e == cudaSuccess) e = sk->jointIndices.upload(d->jointIndices, size_t(d->numVertices) * 4, s);
-    if (e == cudaSuccess) e = sk->weights.upload(d->jointWeights, size_t(d->numVertices) * 4, s);
-    if (e == cudaSuccess && d->normals) e = sk->normals.upload(d->normals, d->numVertices, s);
-    if (e == cudaSuccess && d->tangents) e = sk->tangents.upload(d->tangents, d->numVertices, s);
-    if (e == cudaSuccess) e = sk->outPositions.alloc(size_t(d->numVertices) * 3);
-    if (e == cudaSuccess) e = sk->outNormals.alloc(d->numVertices);
-    if (e == cudaSuccess) e = sk->outTangents.alloc(d->numVertices);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { delete sk; CU(e); }
+    CU(sk->positions.upload(d->positions, size_t(d->numVertices) * 3, s)); CU(sk->jointIndices.upload(d->jointIndices, size_t(d->numVertices) * 4, s)); CU(sk->weights.upload(d->jointWeights, size_t(d->numVertices) * 4, s));
+    if (d->normals) CU(sk->normals.upload(d->normals, d->numVertices, s));
+    if (d->tangents) CU(sk->tangents.upload(d->tangents, d->numVertices, s));
+    CU(sk->outPositions.alloc(size_t(d->numVertices) * 3)); CU(sk->outNormals.alloc(d->numVertices)); CU(sk->outTangents.alloc(d->numVertices));
+    CU(cudaStreamSynchronize(s));
     {   // last frame's positions for the BUILD pass's motion vectors: a geometry that came without a previous-position stream gets a range now, holding its current corners
         const uint32_t subIndex = inst.firstGeometryInstanceIndex + d->geometryIndexInInstance;
         if (c->hPrevPosBase[subIndex] == 0xFFFFFFFFu && sk->numTriangles)
         {
-            e = syncContext(c);
+            CU(syncContext(c));
             DeviceArray<float> grown;
-            if (e == cudaSuccess) e = grown.alloc((c->prevPosTriangles + sk->numTriangles) * 9);
-            if (e == cudaSuccess && c->prevPosTriangles) e = cudaMemcpy(grown.ptr, c->dTriPrevPos.ptr, c->prevPosTriangles * 36, cudaMemcpyDeviceToDevice);
-            if (e != cudaSuccess) { grown.release(); delete sk; CU(e); }
-            c->dTriPrevPos.release(); c->dTriPrevPos = grown; grown.ptr = nullptr; grown.count = 0;
+            CU(grown.alloc((c->prevPosTriangles + sk->numTriangles) * 9));
+            if (c->prevPosTriangles) CU(cudaMemcpy(grown.ptr, c->dTriPrevPos.ptr, c->prevPosTriangles * 36, cudaMemcpyDeviceToDevice));
+            c->dTriPrevPos = std::move(grown);
             c->hPrevPosBase[subIndex] = uint32_t(c->prevPosTriangles); c->prevPosTriangles += sk->numTriangles;
-            e = cudaMemcpy(c->dPrevPosBase.ptr + subIndex, &c->hPrevPosBase[subIndex], 4, cudaMemcpyHostToDevice);
+            CU(cudaMemcpy(c->dPrevPosBase.ptr + subIndex, &c->hPrevPosBase[subIndex], 4, cudaMemcpyHostToDevice));
             skin::Params ip{}; ip.numTriangles = sk->numTriangles; ip.firstGid = sk->firstGid; ip.triShade = c->dTriShade.ptr; ip.triPrevPos = c->dTriPrevPos.ptr + size_t(c->hPrevPosBase[subIndex]) * 9;
-            if (e == cudaSuccess) { launchSkinInitPrev(ip, s); e = cudaStreamSynchronize(s); }
-            if (e != cudaSuccess) { delete sk; CU(e); }
+            launchSkinInitPrev(ip, s); CU(cudaStreamSynchronize(s));
         }
         sk->prevPosFirst = c->hPrevPosBase[subIndex];
     }
-    c->skins.push_back(sk); *outSkinId = uint32_t(c->skins.size() - 1);
+    c->skins.push_back(std::move(sk)); *outSkinId = uint32_t(c->skins.size() - 1);
     return RTXPT_OK;
 }
 extern "C" RTXPT_API int rtxpt_b200_skin_update(rtxpt_ctx* c, uint32_t skinId, const float* jointMatrices4x4, uint32_t numJoints, void* cudaStream)
@@ -1102,20 +1082,17 @@ extern "C" RTXPT_API int rtxpt_b200_bake_env_map(rtxpt_ctx* c, const RtxptEnvBak
     const uint32_t levels = rtxpt_b200_env_bake_mip_count(d->cubeDim);
     DeviceArray<float> src, dst;
     const size_t srcFloats = d->sourceType == 1 ? size_t(d->sourceWidth) * d->sourceHeight * 4 : (d->sourceType == 2 ? size_t(6) * d->sourceWidth * d->sourceWidth * 4 : 0);
-    cudaError_t e = srcFloats ? src.upload(d->source, srcFloats, s) : cudaSuccess;
-    if (e == cudaSuccess) e = dst.alloc(total);
-    if (e != cudaSuccess) { src.release(); dst.release(); CU(e); }
+    if (srcFloats) CU(src.upload(d->source, srcFloats, s));
+    CU(dst.alloc(total));
     envbake::Params p{};
     p.cubeDim = d->cubeDim; p.sourceType = d->sourceType; p.sourceWidth = d->sourceWidth; p.sourceHeight = d->sourceHeight; p.source = src.ptr;
     memcpy(p.scaleColor, d->scaleColor, 12); p.lightCount = d->directionalLightCount;
     for (uint32_t i = 0; i < d->directionalLightCount; i++) { memcpy(p.lights[i].colorIntensity, d->lights[i].colorIntensity, 16); memcpy(p.lights[i].direction, d->lights[i].direction, 12); p.lights[i].angularSize = d->lights[i].angularSize; }
     size_t off = 0; for (uint32_t m = 0; m < levels; m++) { p.mips[m] = dst.ptr + off; off += size_t(6) * (d->cubeDim >> m) * (d->cubeDim >> m) * 4; }
     launchEnvBake(p, levels, s);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, dst.ptr, total * 4, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    src.release(); dst.release();
-    CU(e);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(out, dst.ptr, total * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
     return RTXPT_OK;
 }
 
@@ -1130,7 +1107,7 @@ static int neeatEnsure(rtxpt_ctx* c, cudaStream_t s)
     if (n.allocated && n.host.W == W && n.host.H == H && n.lightCount == L) return RTXPT_OK;
     if (n.allocated && n.host.W == W && n.host.H == H && L <= n.lightCapacity) { n.lightCount = L; return RTXPT_OK; }       // the light list changed length: per-light arrays have headroom, the feedback state stays
     CU(syncContext(c)); CU(cudaStreamSynchronize(s));
-    n.release(); n.host.reset(W, H); n.lightCount = L;
+    n = rtxpt_ctx::Neeat(); n.host.reset(W, H); n.lightCount = L;
     const size_t P = size_t(W) * H, B = size_t((W + 1) / 2) * ((H + 1) / 2), T = size_t(neeat::HostState::tilesX(W)) * neeat::HostState::tilesY(H) * neeat::kLocalProxyCount;
     const uint32_t Lcap = L + 4096u; n.lightCapacity = Lcap;        // headroom for lights added later (rtxpt_b200_update_lights); beyond it the feedback state starts over
     const size_t proxyCapacity = size_t(neeat::kProxyRatio) * std::max<uint32_t>(Lcap, neeat::kMaxLights / 10) + Lcap;           // every light rounds its share up
@@ -1138,12 +1115,12 @@ static int neeatEnsure(rtxpt_ctx* c, cudaStream_t s)
     CU(n.local.alloc(T)); CU(n.counters.alloc(size_t(Lcap) + 1)); CU(n.proxyCounters.alloc(Lcap)); CU(n.proxyOffsets.alloc(size_t(Lcap) + 1)); CU(n.proxyIndices.alloc(proxyCapacity)); CU(n.samplingProxyCount.alloc(1));
     CU(n.scanBlockSums.alloc(1024)); CU(n.lightWeights.alloc(Lcap)); CU(n.rrFix.alloc(c->capacity)); CU(n.shadowFeedback.alloc(c->capacity));
     CU(n.pastToCurrent.alloc(Lcap)); CU(n.currentToPast.alloc(Lcap));
-    CU(cudaMemsetAsync(n.rrFix.ptr, 0, size_t(c->capacity) * 4, s));
-    CU(n.weights[0].alloc(Lcap)); CU(n.weights[1].alloc(Lcap)); CU(n.weightGroupSums.alloc((Lcap + 4095) / 4096 + 1)); CU(n.weightsSum.alloc(1)); n.weightPingPong = 0;
-    CU(cudaMemsetAsync(n.weights[0].ptr, 0, size_t(Lcap) * 4, s)); CU(cudaMemsetAsync(n.weights[1].ptr, 0, size_t(Lcap) * 4, s));
-    CU(cudaMemsetAsync(n.fbWeight.ptr, 0, P * 4, s)); CU(cudaMemsetAsync(n.scratchWeight.ptr, 0, P * 4, s)); CU(cudaMemsetAsync(n.blendedWeight.ptr, 0, B * 4, s)); CU(cudaMemsetAsync(n.historyDepth.ptr, 0, P * 4, s));
-    CU(cudaMemsetAsync(n.fbCandidate.ptr, 0xFF, P * 4, s)); CU(cudaMemsetAsync(n.scratchCandidate.ptr, 0xFF, P * 4, s)); CU(cudaMemsetAsync(n.blendedCandidate.ptr, 0xFF, B * 4, s));
-    CU(cudaMemsetAsync(n.local.ptr, 0, T * 4, s)); CU(cudaMemsetAsync(n.samplingProxyCount.ptr, 0, 4, s));
+    CU(n.rrFix.fill(0, s));
+    CU(n.weights[0].alloc(Lcap)); CU(n.weights[1].alloc(Lcap)); CU(n.weightGroupSums.alloc((Lcap + 4095) / 4096 + 1)); CU(n.weightsSum.alloc(1));
+    CU(n.weights[0].fill(0, s)); CU(n.weights[1].fill(0, s));
+    CU(n.fbWeight.fill(0, s)); CU(n.scratchWeight.fill(0, s)); CU(n.blendedWeight.fill(0, s)); CU(n.historyDepth.fill(0, s));
+    CU(n.fbCandidate.fill(0xFF, s)); CU(n.scratchCandidate.fill(0xFF, s)); CU(n.blendedCandidate.fill(0xFF, s));
+    CU(n.local.fill(0, s)); CU(n.samplingProxyCount.fill(0, s));
     n.allocated = true;
     return RTXPT_OK;
 }
@@ -1186,7 +1163,7 @@ extern "C" RTXPT_API int rtxpt_b200_neeat_reset(rtxpt_ctx* c)
     if (!c) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null context");
     cudaSetDevice(c->device);
     CU(syncContext(c));
-    c->na.release();
+    c->na = rtxpt_ctx::Neeat();
     return RTXPT_OK;
 }
 extern "C" RTXPT_API int rtxpt_b200_neeat_update_begin(rtxpt_ctx* c, void* cudaStream)
@@ -1288,20 +1265,18 @@ static int ensureReblurPools(rtxpt_ctx* c, cudaStream_t s)
     for (auto& h : c->reblur)
     {
         CU(h.prevViewZ.alloc(P)); CU(h.prevNormalRoughness.alloc(P)); CU(h.prevInternalData.alloc(P)); CU(h.diffFast.alloc(P)); CU(h.specFast.alloc(P)); CU(h.diffHistory.alloc(P)); CU(h.specHistory.alloc(P));
-        CU(cudaMemsetAsync(h.prevViewZ.ptr, 0, P * 4, s)); CU(cudaMemsetAsync(h.prevNormalRoughness.ptr, 0, P * 4, s)); CU(cudaMemsetAsync(h.prevInternalData.ptr, 0, P * 2, s)); CU(cudaMemsetAsync(h.diffFast.ptr, 0, P * 2, s));
-        CU(cudaMemsetAsync(h.specFast.ptr, 0, P * 2, s)); CU(cudaMemsetAsync(h.diffHistory.ptr, 0, P * 8, s)); CU(cudaMemsetAsync(h.specHistory.ptr, 0, P * 8, s));
+        CU(h.prevViewZ.fill(0, s)); CU(h.prevNormalRoughness.fill(0, s)); CU(h.prevInternalData.fill(0, s)); CU(h.diffFast.fill(0, s)); CU(h.specFast.fill(0, s)); CU(h.diffHistory.fill(0, s)); CU(h.specHistory.fill(0, s));
         for (int i = 0; i < 2; i++)
         {
             CU(h.tracking[i].alloc(P)); CU(h.diffLuma[i].alloc(P)); CU(h.specLuma[i].alloc(P));
-            CU(cudaMemsetAsync(h.tracking[i].ptr, 0, P * 2, s)); CU(cudaMemsetAsync(h.diffLuma[i].ptr, 0, P * 2, s)); CU(cudaMemsetAsync(h.specLuma[i].ptr, 0, P * 2, s));
+            CU(h.tracking[i].fill(0, s)); CU(h.diffLuma[i].fill(0, s)); CU(h.specLuma[i].fill(0, s));
         }
         h.valid = false; h.pingPong = 0;
     }
     CU(c->rbTiles.alloc(T)); CU(c->rbTmp1Diff.alloc(P)); CU(c->rbTmp1Spec.alloc(P)); CU(c->rbTmp2Diff.alloc(P)); CU(c->rbTmp2Spec.alloc(P)); CU(c->rbOutDiff.alloc(P)); CU(c->rbOutSpec.alloc(P));
     CU(c->rbTrackingT.alloc(P)); CU(c->rbDiffFastT.alloc(P)); CU(c->rbSpecFastT.alloc(P)); CU(c->rbData1.alloc(P)); CU(c->rbData2.alloc(P));
-    CU(cudaMemsetAsync(c->rbTmp1Diff.ptr, 0, P * 8, s)); CU(cudaMemsetAsync(c->rbTmp1Spec.ptr, 0, P * 8, s)); CU(cudaMemsetAsync(c->rbTmp2Diff.ptr, 0, P * 8, s)); CU(cudaMemsetAsync(c->rbTmp2Spec.ptr, 0, P * 8, s));
-    CU(cudaMemsetAsync(c->rbOutDiff.ptr, 0, P * 8, s)); CU(cudaMemsetAsync(c->rbOutSpec.ptr, 0, P * 8, s)); CU(cudaMemsetAsync(c->rbTrackingT.ptr, 0, P * 2, s)); CU(cudaMemsetAsync(c->rbDiffFastT.ptr, 0, P * 2, s));
-    CU(cudaMemsetAsync(c->rbSpecFastT.ptr, 0, P * 2, s)); CU(cudaMemsetAsync(c->rbData1.ptr, 0, P * 2, s)); CU(cudaMemsetAsync(c->rbData2.ptr, 0, P * 4, s));
+    CU(c->rbTmp1Diff.fill(0, s)); CU(c->rbTmp1Spec.fill(0, s)); CU(c->rbTmp2Diff.fill(0, s)); CU(c->rbTmp2Spec.fill(0, s)); CU(c->rbOutDiff.fill(0, s)); CU(c->rbOutSpec.fill(0, s));
+    CU(c->rbTrackingT.fill(0, s)); CU(c->rbDiffFastT.fill(0, s)); CU(c->rbSpecFastT.fill(0, s)); CU(c->rbData1.fill(0, s)); CU(c->rbData2.fill(0, s));
     c->reblurWidth = c->tableWidth; c->reblurHeight = c->tableHeight;
     return RTXPT_OK;
 }
@@ -1338,7 +1313,7 @@ extern "C" RTXPT_API int rtxpt_b200_denoise_realtime(rtxpt_ctx* c, const RtxptDe
     int rc = checkRealtimeReady(c); if (rc != RTXPT_OK) return rc;
     if (!k || !f) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null constants");
     cudaStream_t s = pickStream(c, cudaStream);
-    if (!c->evDnStart) { CU(cudaEventCreate(&c->evDnStart)); CU(cudaEventCreate(&c->evDnStop)); }
+    if (!c->evDnStop) { CU(c->evDnStart.create(cudaEventCreateWithFlags, cudaEventDefault)); CU(c->evDnStop.create(cudaEventCreateWithFlags, cudaEventDefault)); }
     CU(cudaEventRecord(c->evDnStart, s));
     rc = rtxpt_b200_denoise_spec_hit_t(c, cudaStream); if (rc != RTXPT_OK) return rc;          // "Denoising Guides Bake" precedes Sample::Denoise in the frame
     bool first = true;
@@ -1616,10 +1591,9 @@ extern "C" RTXPT_API int rtxpt_b200_trace_rays(rtxpt_ctx* c, const RtxptRay* ray
     cudaSetDevice(c->device);
     DeviceArray<RtxptRay> dRays; DeviceArray<RtxptHit> dHits;
     CU(dRays.upload(rays, count, c->stream)); CU(dHits.alloc(count));
-    int rc = rtxpt_b200_trace_rays_device(c, dRays.ptr, count, anyHit, dHits.ptr, 1, nullptr);
-    if (rc == RTXPT_OK) { cudaError_t e = cudaMemcpy(outHits, dHits.ptr, size_t(count) * sizeof(RtxptHit), cudaMemcpyDeviceToHost); if (e != cudaSuccess) rc = fail(RTXPT_ERR_CUDA, "readback failed: %s", cudaGetErrorString(e)); }
-    dRays.release(); dHits.release();
-    return rc;
+    int rc = rtxpt_b200_trace_rays_device(c, dRays.ptr, count, anyHit, dHits.ptr, 1, nullptr); if (rc != RTXPT_OK) return rc;
+    CU(cudaMemcpy(outHits, dHits.ptr, size_t(count) * sizeof(RtxptHit), cudaMemcpyDeviceToHost));
+    return RTXPT_OK;
 }
 
 extern "C" RTXPT_API int rtxpt_b200_set_view(rtxpt_ctx* c, const RtxptViewConstants* view)
@@ -1662,7 +1636,6 @@ extern "C" RTXPT_API int rtxpt_b200_debug_bsdf(rtxpt_ctx* c, const float* in, ui
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(out, dOut.ptr, size_t(count) * 16 * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     CU(syncContext(c));
-    dIn.release(); dOut.release();
     return RTXPT_OK;
 }
 
@@ -1676,6 +1649,12 @@ extern "C" RTXPT_API int rtxpt_b200_debug_rng(rtxpt_ctx* c, const uint32_t* in, 
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(out, dOut.ptr, size_t(count) * 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CU(syncContext(c));
-    dIn.release(); dOut.release();
+    return RTXPT_OK;
+}
+
+extern "C" RTXPT_API int rtxpt_b200_debug_live_resources(uint64_t* out)
+{
+    if (!out) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    *out = g_liveResources.load();
     return RTXPT_OK;
 }

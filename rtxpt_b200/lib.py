@@ -74,6 +74,7 @@ _SIGNATURES = {
     "rtxpt_b200_get_lights_ex": [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)],
     "rtxpt_b200_debug_bsdf": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p],
     "rtxpt_b200_debug_rng": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p],
+    "rtxpt_b200_debug_live_resources": [C.POINTER(C.c_uint64)],
 }
 _LOADER_SYMBOLS = ["rtxpt_b200_debug_decode_jpeg", "rtxpt_b200_debug_decode_jpeg_error", "rtxpt_b200_load_hdr_image", "rtxpt_b200_load_hdr_image_error", "rtxpt_b200_loader_keep_block_compression", "rtxpt_b200_load_dds_hdr", "rtxpt_b200_host_opacity_micro_index", "rtxpt_b200_camera_matrices", "rtxpt_b200_tone_map_pre_exposed_gray", "rtxpt_b200_debug_build_bvh", "rtxpt_b200_env_bake_mip_count", "rtxpt_b200_env_bake_floats", "rtxpt_b200_load_gltf", "rtxpt_b200_load_gltf_ex", "rtxpt_b200_load_scene_json", "rtxpt_b200_host_scene_info", "rtxpt_b200_load_gltf_error", "rtxpt_b200_host_scene_desc", "rtxpt_b200_host_scene_cameras",
                    "rtxpt_b200_host_scene_triangle_count", "rtxpt_b200_free_host_scene", "rtxpt_b200_bridge_camera", "rtxpt_b200_default_constants", "rtxpt_b200_debug_bvh_stats", "rtxpt_b200_parse_material_json", "rtxpt_b200_parse_material_json_error", "rtxpt_b200_debug_decode_dds", "rtxpt_b200_debug_decode_dds_error",
