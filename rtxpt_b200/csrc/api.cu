@@ -126,6 +126,7 @@ struct rtxpt_ctx
     DeviceArray<LightInfo> dLights; DeviceArray<uint32_t> dProxyCounters, dProxyIndices, dEnvLookup; DeviceArray<uint4> dLightsEx;
     // wavefront
     DeviceArray<uint4> s0, s1, s2, s3, s4; DeviceArray<float4> hits; DeviceArray<uint32_t> rayQueue[2], shadeQueue;
+    DeviceArray<uint4> t0, t1, t2, t3, t4; DeviceArray<uint2> radiance;        // reference mode: second path-state set, radiance per home index (wavefront.cuh)
     DeviceArray<float4> shadowOriginTMax, shadowDirPath; DeviceArray<uint2> shadowRadiance;
     DeviceArray<uint32_t> counters; DeviceArray<uint32_t> pixelOfSlot, allPixelTable;
     uint32_t paddedPixelsPerRank = 0;
@@ -571,6 +572,7 @@ static int ensureTargets(rtxpt_ctx* c, uint32_t W, uint32_t H)
     if (cap >= 0x7FFFFFFFull) return fail(RTXPT_ERR_UNSUPPORTED, "too many path slots");
     c->capacity = uint32_t(std::max<size_t>(cap, 1));
     CU(c->s0.alloc(c->capacity)); CU(c->s1.alloc(c->capacity)); CU(c->s2.alloc(c->capacity)); CU(c->s3.alloc(c->capacity)); CU(c->s4.alloc(c->capacity));
+    CU(c->t0.alloc(c->capacity)); CU(c->t1.alloc(c->capacity)); CU(c->t2.alloc(c->capacity)); CU(c->t3.alloc(c->capacity)); CU(c->t4.alloc(c->capacity)); CU(c->radiance.alloc(c->capacity));
     CU(c->hits.alloc(c->capacity)); CU(c->rayQueue[0].alloc(c->capacity)); CU(c->rayQueue[1].alloc(c->capacity));
     CU(c->shadeQueue.alloc(size_t(c->capacity) * kNumShadeClasses));
     CU(c->shadowOriginTMax.alloc(c->capacity)); CU(c->shadowDirPath.alloc(c->capacity)); CU(c->shadowRadiance.alloc(c->capacity));
@@ -627,6 +629,7 @@ static void fillParams(rtxpt_ctx* c, LaunchParams& p)
     w.rayQueue[0] = c->rayQueue[0].ptr; w.rayQueue[1] = c->rayQueue[1].ptr; w.shadeQueue = c->shadeQueue.ptr;
     w.shadowOriginTMax = c->shadowOriginTMax.ptr; w.shadowDirPath = c->shadowDirPath.ptr; w.shadowRadiance = c->shadowRadiance.ptr;
     w.counters = c->counters.ptr; w.pixelOfSlot = c->pixelOfSlot.ptr; w.capacity = c->capacity; w.pixelCount = c->pixelCount;
+    p.stateIn = StateSet{ c->s0.ptr, c->s1.ptr, c->s2.ptr, c->s3.ptr, c->s4.ptr }; p.stateOut = StateSet{ c->t0.ptr, c->t1.ptr, c->t2.ptr, c->t3.ptr, c->t4.ptr }; p.radiance = c->radiance.ptr;
     p.c = c->consts;
     p.flags = c->cfg.flags;
     p.refillThreshold = c->tune.refillThreshold; p.waitFlushLanes = c->tune.waitFlushLanes;
@@ -720,6 +723,8 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
                 w.s0 += o; w.s1 += o; w.s2 += o; w.s3 += o; w.s4 += o; w.hits += o; w.rayQueue[0] += o; w.rayQueue[1] += o; w.shadeQueue += o * kNumShadeClasses;
                 w.shadowOriginTMax += o; w.shadowDirPath += o; w.shadowRadiance += o; w.counters += size_t(l) * kCounterWords; w.capacity = uint32_t(std::max<size_t>(size_t(count) * c->pixelCount, 1));
                 if (na) { q.naShadowFeedback += o; q.naRrFix += o; }
+                for (StateSet* st : { &q.stateIn, &q.stateOut }) { st->s0 += o; st->s1 += o; st->s2 += o; st->s3 += o; st->s4 += o; }
+                q.radiance += o;
             }
             q.firstSampleIndex = c->consts.sampleBaseIndex + firstSubSampleIndex + done + firstSub;
             q.subSampleCount = count;
@@ -728,12 +733,13 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
             q.iteration = 0;
             KernelTimer ktl{ c, ls, kt.on };
             ktl.begin(3); launchGenerate(q, c->grid, ls); ktl.end(); launches++;
-            // Shadow rays of vertex k and scatter rays of vertex k+1 touch disjoint state (shadow: shadow records + the radiance word of the path;
-            // closest: ray words, hit records, shade queues), so k_trace_shadow(it) runs on a second stream next to k_trace_closest(it+1): the
+            // Shadow rays of vertex k and scatter rays of vertex k+1 touch disjoint state (shadow: shadow records + the path's radiance at its home index;
+            // closest: ray words of the state set, hit records, shade queues), so k_trace_shadow(it) runs on a second stream next to k_trace_closest(it+1): the
             // long-ray tail of one persistent kernel is filled by the other's CTAs.  k_shade(it+1) joins both.
             for (uint32_t it = 0; it < iterations; it++)
             {
                 q.iteration = it;
+                if (it > 0) std::swap(q.stateIn, q.stateOut);     // the paths k_shade(it - 1) appended are iteration it's rays
                 ktl.begin(0); launchTraceClosest(q, c->grid, countSteps, ls); ktl.end();
                 if (overlap && it > 0) CU(cudaStreamWaitEvent(ls, L.evShadowDone, 0));        // shadow(it-1) has updated the radiance words
                 ktl.begin(2); if (na) launchShadeNeeat(q, c->grid, ls); else launchShade(q, c->grid, ls); ktl.end();
@@ -832,7 +838,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
     for (uint32_t it = 0; it < buildIterations; it++)
     {
         p.iteration = it;
-        launchTraceClosest(p, c->grid, false, s); launchRtShade(p, c->grid, false, s); launches += 2;
+        launchTraceClosestRealtime(p, c->grid, s); launchRtShade(p, c->grid, false, s); launches += 2;
     }
     if (na)
     {   // LightsBaker::UpdateEnd sits between the BUILD pass (this frame's depth and motion vectors) and the radiance passes (Sample.cpp:2495)
@@ -851,7 +857,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
         for (uint32_t it = 0; it < fillIterations; it++)
         {
             p.iteration = it;
-            launchTraceClosest(p, c->grid, false, s);
+            launchTraceClosestRealtime(p, c->grid, s);
             if (na) { launchRtShadeNeeat(p, c->grid, s); launchTraceShadowRealtimeNeeat(p, c->grid, s); }
             else { launchRtShade(p, c->grid, true, s); launchTraceShadowRealtime(p, c->grid, s); }
             launches += 3;

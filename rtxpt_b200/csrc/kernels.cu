@@ -69,8 +69,8 @@ __global__ void __launch_bounds__(256) k_generate(const __grid_constant__ Launch
         float3 origin, dir; computeCameraRay(p.c, id, sampleIndex, origin, dir);
         if (p.exportGuides && sub + 1 == p.subSampleCount) p.depth[size_t(py) * p.c.imageWidth + px] = 0.0f;       // Bridge::ExportSurfaceInit
         path.origin = origin; path.dir = dir;
-        path.store(p.wf, slot);
-        p.wf.rayQueue[0][slot] = slot | (path.hasFlag(kPFTerminateAtNextBounce) ? 0x80000000u : 0u);
+        path.storeRay(p.stateIn, slot, slot);          // iteration 0: ray index == home index
+        path.storeRadiance(p.radiance, slot);
     }
 }
 
@@ -87,7 +87,8 @@ constexpr uint kTraceThreads = PT_TRACE_THREADS, kTraceCtaScale = 256 / PT_TRACE
 constexpr uint kTraceWarps = kTraceThreads / 32;
 constexpr uint kTraceScratchBytes = 16 + kTraceWarps * sizeof(WarpScratch);
 
-template <bool COUNT, int MINB>
+// RAY_ORDER (reference mode): ray i is entry i of p.stateIn and writes hits[i]; otherwise (realtime) the ray queue names the path slot
+template <bool COUNT, int MINB, bool RAY_ORDER>
 __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_closest(const __grid_constant__ LaunchParams p)
 {
     extern __shared__ __align__(16) unsigned char smemRaw[];
@@ -145,9 +146,18 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
                 if (i >= count) exhausted = true;
                 else
                 {
-                    entry = queue[i];
-                    const uint slot = entry & 0x7FFFFFFFu;
-                    const uint4 a = ldState(p.wf.s0 + slot), b = ldState(p.wf.s1 + slot);
+                    uint4 a, b;
+                    if constexpr (RAY_ORDER)
+                    {   // the sign bit of s1.w is the path's kPFTerminateAtNextBounce (wavefront.cuh)
+                        a = ldState(p.stateIn.s0 + i); b = ldState(p.stateIn.s1 + i);
+                        entry = i | (b.w & 0x80000000u);
+                    }
+                    else
+                    {
+                        entry = queue[i];
+                        const uint slot = entry & 0x7FFFFFFFu;
+                        a = ldState(p.wf.s0 + slot); b = ldState(p.wf.s1 + slot);
+                    }
                     tv.init(p.scene, ws, mk3(__uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z)), mk3(__uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z)), 0.0f, kMaxRayTravel);
                     hasRay = true;
                 }
@@ -195,18 +205,24 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
                 const float rx = f16tof32(r.x & 0x7FFFu), ry = f16tof32((r.x >> 16) & 0x7FFFu), rz = f16tof32(r.y), rw = f16tof32(r.y >> 16);
                 if (rx > 0 || ry > 0 || rz > 0 || rw > 0)
                 {
-                    uint4 s2 = p.wf.s2[slot];
-                    float lx, ly, lz, lw;
-                    if (REALTIME)
+                    if constexpr (REALTIME)
                     {
+                        uint4 s2 = p.wf.s2[slot];
                         const float a = p.rt.attenuation;
                         const float spec = (r.x & 0x00008000u) ? rw : ((r.x & 0x80000000u) ? (rx + ry + rz) / 3.0f : 0.0f);
-                        lx = f16tof32(s2.z) + rx * a; ly = f16tof32(s2.z >> 16) + ry * a; lz = f16tof32(s2.w) + rz * a; lw = f16tof32(s2.w >> 16) + spec * a;
+                        const float lx = f16tof32(s2.z) + rx * a, ly = f16tof32(s2.z >> 16) + ry * a, lz = f16tof32(s2.w) + rz * a, lw = f16tof32(s2.w >> 16) + spec * a;
+                        s2.z = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
+                        s2.w = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
+                        p.wf.s2[slot] = s2;
                     }
-                    else { lx = f16tof32(s2.z) + rx; ly = f16tof32(s2.z >> 16) + ry; lz = f16tof32(s2.w) + rz; lw = f16tof32(s2.w >> 16); }
-                    s2.z = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
-                    s2.w = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
-                    p.wf.s2[slot] = s2;
+                    else
+                    {   // reference mode: `slot` is the path's home index h
+                        uint2 l = p.radiance[slot];
+                        const float lx = f16tof32(l.x) + rx, ly = f16tof32(l.x >> 16) + ry, lz = f16tof32(l.y) + rz, lw = f16tof32(l.y >> 16);
+                        l.x = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
+                        l.y = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
+                        p.radiance[slot] = l;
+                    }
                 }
                 if constexpr (NEEAT)
                 {   // the light was visible: the pixel's feedback reservoir hears about it (PathTracerNEE.hlsli:276-283) and the path's next shade takes the roulette
@@ -266,9 +282,9 @@ __global__ void __launch_bounds__(256) k_commit_accumulate(const __grid_constant
         uint2 last = make_uint2(0, 0);
         for (uint s = 0; s < p.subSampleCount; s++)
         {
-            const uint4 s2 = p.wf.s2[s * p.wf.pixelCount + pix];
-            const float r = f16tof32(s2.z), g = f16tof32(s2.z >> 16), b = f16tof32(s2.w);
-            last = make_uint2(s2.z, (s2.w & 0xFFFFu) | (0x3C00u << 16));          // float4(L.rgb, 1) as RGBA16F
+            const uint2 l = p.radiance[s * p.wf.pixelCount + pix];
+            const float r = f16tof32(l.x), g = f16tof32(l.x >> 16), b = f16tof32(l.y);
+            last = make_uint2(l.x, (l.y & 0xFFFFu) | (0x3C00u << 16));          // float4(L.rgb, 1) as RGBA16F
             if (p.doAccumulate)
             {   // blend = 1/(n+1); lerp(prev, sample, blend) unless blend >= 1 (Sample.cpp:2775, AccumulationPass.hlsl:57-65)
                 const float blend = 1.0f / (float(n) + 1.0f);
@@ -420,7 +436,8 @@ cudaError_t configureKernels(int maxSmemOptin)
     cudaError_t e;
     const int want = maxSmemOptin > 0 ? maxSmemOptin : 0;
 #define ALLOW(k) if ((e = allowSmem(k, want)) != cudaSuccess) return e
-    ALLOW((k_trace_closest<false, 2>)); ALLOW((k_trace_closest<false, 3>)); ALLOW((k_trace_closest<false, 4>)); ALLOW((k_trace_closest<true, 2>));
+    ALLOW((k_trace_closest<false, 2, true>)); ALLOW((k_trace_closest<false, 3, true>)); ALLOW((k_trace_closest<false, 4, true>)); ALLOW((k_trace_closest<true, 2, true>));
+    ALLOW((k_trace_closest<false, 2, false>)); ALLOW((k_trace_closest<false, 3, false>)); ALLOW((k_trace_closest<false, 4, false>));
     ALLOW((k_trace_shadow<false, 2>)); ALLOW((k_trace_shadow<false, 3>)); ALLOW((k_trace_shadow<false, 4>)); ALLOW((k_trace_shadow<true, 2>));
     ALLOW((k_trace_shadow<false, 4, true>)); ALLOW((k_trace_shadow<false, 2, true>));
     ALLOW((k_trace_shadow<false, 4, true, true>)); ALLOW((k_trace_shadow<false, 2, true, true>)); ALLOW((k_trace_shadow<false, 4, false, true>)); ALLOW((k_trace_shadow<false, 2, false, true>));
@@ -449,10 +466,17 @@ void launchGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) 
 void launchTraceClosest(const LaunchParams& p, const GridConfig& g, bool count, cudaStream_t s)
 {
     const int grid = g.smCount * g.traceBlocksPerSM; const size_t smem = traceSmemBytes(p);
-    if (count) launchTrace(k_trace_closest<true, 2>, grid, smem, s, p, g);
-    else if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_closest<false, 4>, grid, smem, s, p, g);
-    else if (g.traceBlocksPerSM == 3) launchTrace(k_trace_closest<false, 3>, grid, smem, s, p, g);
-    else launchTrace(k_trace_closest<false, 2>, grid, smem, s, p, g);
+    if (count) launchTrace(k_trace_closest<true, 2, true>, grid, smem, s, p, g);
+    else if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_closest<false, 4, true>, grid, smem, s, p, g);
+    else if (g.traceBlocksPerSM == 3) launchTrace(k_trace_closest<false, 3, true>, grid, smem, s, p, g);
+    else launchTrace(k_trace_closest<false, 2, true>, grid, smem, s, p, g);
+}
+void launchTraceClosestRealtime(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
+{
+    const int grid = g.smCount * g.traceBlocksPerSM; const size_t smem = traceSmemBytes(p);
+    if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_closest<false, 4, false>, grid, smem, s, p, g);
+    else if (g.traceBlocksPerSM == 3) launchTrace(k_trace_closest<false, 3, false>, grid, smem, s, p, g);
+    else launchTrace(k_trace_closest<false, 2, false>, grid, smem, s, p, g);
 }
 void launchTraceShadow(const LaunchParams& p, const GridConfig& g, bool count, cudaStream_t s)
 {

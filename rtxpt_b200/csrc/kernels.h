@@ -15,13 +15,14 @@ struct GridConfig
 cudaError_t configureKernels(int maxSmemOptin);
 void queryOccupancy(GridConfig& g, size_t traceSmemBytes);
 void launchGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
-void launchTraceClosest(const LaunchParams& p, const GridConfig& g, bool countSteps, cudaStream_t s);
+void launchTraceClosest(const LaunchParams& p, const GridConfig& g, bool countSteps, cudaStream_t s);           // reference mode: rays in state order
 void launchShade(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchTraceShadow(const LaunchParams& p, const GridConfig& g, bool countSteps, cudaStream_t s);
 // realtime mode (realtime_kernels.cu; the shadow kernel variant lives with the other traversal kernels)
 void launchRtBuildGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtFillGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtShade(const LaunchParams& p, const GridConfig& g, bool fill, cudaStream_t s);
+void launchTraceClosestRealtime(const LaunchParams& p, const GridConfig& g, cudaStream_t s);                    // realtime mode: rays through the slot queue
 void launchTraceShadowRealtime(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtFillCommit(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s);

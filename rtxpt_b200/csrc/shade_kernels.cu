@@ -12,30 +12,20 @@
 
 namespace pt {
 
-// warp-aggregated append of `value` to queue region `cls` (0xFF = nothing to append); every lane of the warp must call this
-PT_DEVICE void warpAppend(uint* queueBase, uint regionStride, uint* counters, uint cls, uint value)
+// warp-aggregated append to counter `cls` (0xFF = nothing to append); every lane of the warp must call this.  Returns the lane's position.
+PT_DEVICE uint warpAppend(uint* counters, uint cls)
 {
     const uint lane = threadIdx.x & 31u;
     const uint peers = __match_any_sync(0xFFFFFFFFu, cls);
+    uint base = 0;
     if (cls != 0xFFu)
     {
         const uint leader = __ffs(peers) - 1u;
-        uint base = 0;
         if (lane == leader) base = atomicAdd(counters + cls, __popc(peers));
-        base = __shfl_sync(peers, base, leader);
-        queueBase[size_t(cls) * regionStride + base + __popc(peers & ((1u << lane) - 1u))] = value;
+        base = __shfl_sync(peers, base, leader) + __popc(peers & ((1u << lane) - 1u));
     }
+    return base;
 }
-
-// next-item prefetch in k_shade: 0 off, 1 into L2, 2 into L1
-#ifndef PT_SHADE_PREFETCH
-#define PT_SHADE_PREFETCH 0
-#endif
-#if PT_SHADE_PREFETCH == 2
-#define PT_PREFETCH(ptr) asm volatile("prefetch.global.L1 [%0];" ::"l"(ptr))
-#else
-#define PT_PREFETCH(ptr) asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr))
-#endif
 
 __global__ void k_init_sobol_tables()
 {
@@ -53,60 +43,32 @@ __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ Lau
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
     uint* ctrNext = ctr + kCountersPerIter;
-    uint* nextQueue = p.wf.rayQueue[(p.iteration + 1) & 1];
     const uint warpsPerBlock = blockDim.x >> 5, lane = threadIdx.x & 31u;
     const uint warpGlobal = blockIdx.x * warpsPerBlock + (threadIdx.x >> 5), warpStride = gridDim.x * warpsPerBlock;
     for (int cls = 0; cls < kNumShadeClasses; cls++)
     {
         const uint count = ctr[kCtrShadeCount + cls];
         const uint* __restrict__ queue = p.wf.shadeQueue + size_t(cls) * p.wf.capacity;
-#if PT_SHADE_PREFETCH
-        // Software pipeline over the queue (the kernel is latency-bound: 4 warps per scheduler, a chain of dependent gathers per path): while
-        // item k is shaded, the state words and the hit of item k+1 are pulled towards the SM, and once its hit has arrived, its 96-byte shade record.
-        uint slotNext = (warpGlobal * 32u + lane < count) ? queue[warpGlobal * 32u + lane] : 0xFFFFFFFFu;
-#endif
         for (uint base = warpGlobal * 32u; base < count; base += warpStride * 32u)
         {
             const uint i = base + lane;
-            uint rayCls = 0xFFu, shadowCls = 0xFFu, rayEntry = 0, slot = 0;
+            uint rayCls = 0xFFu, shadowCls = 0xFFu, h = 0;
+            PathRegs path;
             HitOutputs out; out.continuePath = false; out.emitShadow = false;
-#if PT_SHADE_PREFETCH
-            const uint slotNow = slotNext;
-            { const uint ni = i + warpStride * 32u; slotNext = ni < count ? queue[ni] : 0xFFFFFFFFu; }          // consumed after this item: the load has a whole item to land
-#endif
             if (i < count)
             {
-#if PT_SHADE_PREFETCH
-                slot = slotNow;
-#else
-                slot = queue[i];
-#endif
-                PathRegs path; path.load(p.wf, slot, true);
+                const uint r = queue[i];
+                h = path.loadRay(p.stateIn, r, p.radiance);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
-#if PT_SHADE_PREFETCH
-                const float4 hitNow = cls != 0 ? p.wf.hits[slot] : make_float4(0.f, 0.f, 0.f, 0.f);
-                if (slotNext != 0xFFFFFFFFu)
-                {   // next item's state and hit (its slot index was loaded an item ago)
-                    PT_PREFETCH(p.wf.s0 + slotNext); PT_PREFETCH(p.wf.s1 + slotNext); PT_PREFETCH(p.wf.s2 + slotNext); PT_PREFETCH(p.wf.s3 + slotNext); PT_PREFETCH(p.wf.s4 + slotNext);
-                    if (cls != 0) PT_PREFETCH(p.wf.hits + slotNext);
-                }
                 if (cls == 0) shadeMiss<EXPORT_GUIDES, kModeReference, NEEAT>(p, path);
-                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT>(p, path, slot, hitNow, out);
-                if (cls != 0 && slotNext != 0xFFFFFFFFu)
-                {   // by now the next hit is close: its triangle's shade record (96 B = one or two 128-byte lines)
-                    const uint gidNext = __float_as_uint(p.wf.hits[slotNext].w);
-                    const uint4* rec = p.scene.triShade + size_t(gidNext) * kTriShadeWords;
-                    PT_PREFETCH(rec); PT_PREFETCH(rec + 5);
-                }
-#else
-                if (cls == 0) shadeMiss<EXPORT_GUIDES, kModeReference, NEEAT>(p, path);
-                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT>(p, path, slot, p.wf.hits[slot], out);
-#endif
-                if (cls != 0 && out.continuePath) path.store(p.wf, slot); else path.storeRadianceOnly(p.wf, slot);
-                if (out.continuePath) { rayCls = 0; rayEntry = slot | (path.hasFlag(kPFTerminateAtNextBounce) ? 0x80000000u : 0u); }
+                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT>(p, path, h, p.wf.hits[r], out);
+                path.storeRadiance(p.radiance, h);
+                if (out.continuePath) rayCls = 0;
                 if (out.emitShadow) shadowCls = 0;
             }
-            warpAppend(nextQueue, 0, ctrNext + kCtrRayCount, rayCls, rayEntry);
+            // a continuing path becomes a ray of the next iteration: appended to the other state set, so a warp's paths land in consecutive entries
+            const uint next = warpAppend(ctrNext + kCtrRayCount, rayCls);
+            if (rayCls == 0) path.storeRay(p.stateOut, next, h);
             // shadow records: warp-aggregated, long rays from the front of the three arrays, the rest from the back (appendShadowRecord)
             {
                 const uint b = appendShadowRecord(p, ctr, shadowCls == 0, out.shadow.originTMax.w);

@@ -1,11 +1,19 @@
 // wavefront.cuh — per-path state in HBM (structure of arrays), queues and launch parameters of the wavefront path tracer.
 //
 // The reference keeps an 80-byte PathState in the DXR payload of a megakernel (Rtxpt/Shaders/PathTracer/PathState.hlsli:83-121,
-// PathPayload.hlsli:19-27).  Here the same 80 bytes live in five uint4 arrays indexed by path slot, so that every kernel of the
-// wavefront reads/writes whole 16-byte words that are contiguous across a warp whenever the queue is contiguous:
-//   s0: origin.xyz, id            s1: dir.xyz, sceneLength          s2: thp(fp16 x4), L(fp16 x4)
+// PathPayload.hlsli:19-27).  Here the same 80 bytes live in five uint4 arrays (structure of arrays), so that every kernel of the
+// wavefront reads/writes whole 16-byte words that are contiguous across a warp whenever the indices are:
+//   s0: origin.xyz, id            s1: dir.xyz, sceneLength          s2: thp(fp16 x4), L(fp16 x4)   (reference mode: thp, h, 0)
 //   s3: interiorList[0..1], packedCounters, rayCone(fp16 x2)        s4: fireflyK|bsdfPdf, misInfo|ruRuCorrection, flagsAndVertexIndex, sampleIndex
 // (stableBranchID of the reference payload is unused in reference mode; its word carries the path's sample index instead.)
+//
+// Reference mode keeps the state in ray order: iteration i's rays are entries 0..count-1 of state set i & 1 (LaunchParams::stateIn), and
+// k_shade appends each continuing path to the other set (stateOut) with a warp-aggregated counter, so the ray index is the position and
+// every kernel reads and writes the state in whole, contiguous sectors.  Only the radiance stays at the path's home index
+// h = sub-sample * pixelCount + pixel slot (LaunchParams::radiance, fp16 x4): the shadow kernel adds to it while the next iteration's
+// closest-hit kernel already runs, and the commit kernel reads it per pixel.  s2 carries h in place of L, and s1.w carries
+// kPFTerminateAtNextBounce in its sign bit (sceneLength is never negative) so that the closest-hit kernel bins terminating paths from the
+// words it reads anyway.  Realtime mode indexes one state set by path slot through its ray queues.
 #pragma once
 #include "device_math.cuh"
 #include "neeat.cuh"
@@ -19,16 +27,18 @@ constexpr int kMaxWavefrontIterations = 64;   // reference mode needs bounceCoun
 struct ShadowRecord         // 40 bytes in three arrays
 {
     float4 originTMax;      // ComputeVisibilityRay origin, shortened tMax
-    float4 dirPath;         // direction, path slot (as bits)
+    float4 dirPath;         // direction, path slot (realtime) or home index h (reference mode) as bits
     uint2  radiance;        // NEEResult::RadianceAndSpecAvgPkg (fp16 x4): what L gains if the light is visible
 };
 
+struct StateSet { uint4* s0; uint4* s1; uint4* s2; uint4* s3; uint4* s4; };
+
 struct WavefrontBuffers
 {
-    uint4* s0; uint4* s1; uint4* s2; uint4* s3; uint4* s4;
-    float4* hits;                   // t,u,v,gid per path slot
-    uint* rayQueue[2];              // path slots whose scatter ray is to be traced (ping-pong per iteration)
-    uint* shadeQueue;               // kNumShadeClasses regions of `capacity` entries
+    uint4* s0; uint4* s1; uint4* s2; uint4* s3; uint4* s4;     // realtime mode's state, per path slot (reference mode: state set 0)
+    float4* hits;                   // t,u,v,gid per path slot (reference mode: per ray)
+    uint* rayQueue[2];              // realtime mode: path slots whose scatter ray is to be traced (ping-pong per iteration)
+    uint* shadeQueue;               // kNumShadeClasses regions of `capacity` entries: ray indices (reference mode) or path slots (realtime)
     float4* shadowOriginTMax; float4* shadowDirPath; uint2* shadowRadiance;
     uint* counters;                 // see Counter* below, one block per iteration
     const uint* pixelOfSlot;        // packed (x<<16)|y of the pixels this context renders (tile partition), per pixel slot
@@ -102,7 +112,11 @@ struct LaunchParams
     // NEE-AT temporal feedback (kernels instantiated with NEEAT = true only; appended so that every other kernel's parameter offsets stay what they were)
     neeat::Params na;
     uint4* naShadowFeedback;        // per shadow record: light | ssc << 31, feedback weight, reservoir random, Russian roulette outcome had the sample been visible
-    uint* naRrFix;                  // per path slot: set by the shadow kernel when the sample was visible, consumed by the next shade of the path
+    uint* naRrFix;                  // per home index h: set by the shadow kernel when the sample was visible, consumed by the next shade of the path
+    // reference mode's ray-ordered state (see the top of this file; appended for the same reason): the set this iteration's rays are read from,
+    // the set its continuing paths are appended to, and the radiance per home index h
+    StateSet stateIn, stateOut;
+    uint2* radiance;
 };
 
 // every lane of the warp calls this; `emit` lanes get the index of their shadow record
@@ -200,6 +214,28 @@ struct PathRegs             // one path's state in registers
     }
     // a path that ends at this vertex is only read again for its radiance (shadow kernel, commit): 16 of the 80 bytes
     PT_DEVICE void storeRadianceOnly(const WavefrontBuffers& w, uint slot) const { stState(w.s2 + slot, make_uint4(thpXY, thpZ, lXY, lZW)); }
+    // reference mode: ray r of a state set; returns the path's home index h, whose radiance L is loaded from `radiance`
+    PT_DEVICE uint loadRay(const StateSet& st, uint r, const uint2* radiance)
+    {
+        const uint4 a = ldState(st.s0 + r), b = ldState(st.s1 + r), c = ldState(st.s2 + r), d = ldState(st.s3 + r), e = ldState(st.s4 + r);
+        origin = mk3(__uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z)); id = a.w;
+        dir = mk3(__uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z)); sceneLength = __uint_as_float(b.w & 0x7FFFFFFFu);
+        thpXY = c.x; thpZ = c.y;
+        interior0 = d.x; interior1 = d.y; packedCounters = d.z; rayCone = d.w;
+        pack0 = e.x; pack1 = e.y; flagsAndVertexIndex = e.z; sampleIndex = e.w;
+        const uint2 l = radiance[c.z]; lXY = l.x; lZW = l.y;
+        return c.z;
+    }
+    PT_DEVICE void storeRay(const StateSet& st, uint r, uint h) const
+    {
+        const uint terminate = hasFlag(kPFTerminateAtNextBounce) ? 0x80000000u : 0u;
+        stState(st.s0 + r, make_uint4(__float_as_uint(origin.x), __float_as_uint(origin.y), __float_as_uint(origin.z), id));
+        stState(st.s1 + r, make_uint4(__float_as_uint(dir.x), __float_as_uint(dir.y), __float_as_uint(dir.z), __float_as_uint(sceneLength) | terminate));
+        stState(st.s2 + r, make_uint4(thpXY, thpZ, h, 0u));
+        stState(st.s3 + r, make_uint4(interior0, interior1, packedCounters, rayCone));
+        stState(st.s4 + r, make_uint4(pack0, pack1, flagsAndVertexIndex, sampleIndex));
+    }
+    PT_DEVICE void storeRadiance(uint2* radiance, uint h) const { radiance[h] = make_uint2(lXY, lZW); }
     PT_DEVICE float3 thp() const { return mk3(f16tof32(thpXY), f16tof32(thpXY >> 16), f16tof32(thpZ)); }
     PT_DEVICE void setThp(float3 t) { thpXY = packHalf2NoClamp(clampf(t.x, 0.f, kHalfMax), clampf(t.y, 0.f, kHalfMax)); thpZ = packHalf2NoClamp(clampf(t.z, 0.f, kHalfMax), 0.f); }
     PT_DEVICE float4 L() const { return make_float4(f16tof32(lXY), f16tof32(lXY >> 16), f16tof32(lZW), f16tof32(lZW >> 16)); }
