@@ -414,11 +414,19 @@ RTXPT_API int rtxpt_b200_tone_map_pre_exposed_gray(const RtxptToneMappingParams*
 
 /* ---- Rigid-instance animation (SURVEY §8f row 4; stands in for the per-frame BLAS / TLAS update behind Sample::UpdateAccelStructs and BuildTLAS, Rtxpt/Sample.cpp:1170-1240): new
  * row-major 3x4 matrices for every instance of the uploaded scene; on the stream, the leaf triangles are re-transformed (one thread each) and the 8-wide BVH is refitted bottom-up,
- * level by level, with the builder's own quantisation - unmoved geometry gives back the built nodes bit for bit, topology never changes (quality degrades with large deformation,
- * re-upload then).  The instance table keeps the previous call's matrices as InstanceData.prevTransform: the BUILD pass's motion vectors are those of the moved surface (BridgeDonut:631,
+ * level by level, with the builder's own quantisation - unmoved geometry gives back the built nodes bit for bit, topology never changes (quality degrades with large deformation:
+ * rtxpt_b200_rebuild_bvh then).  The instance table keeps the previous call's matrices as InstanceData.prevTransform: the BUILD pass's motion vectors are those of the moved surface (BridgeDonut:631,
  * PathTracerStablePlanes.hlsli:282-291); call it every frame, as Sample does its TLAS update, so that an instance that stopped reports no motion.  Emissive triangles are baked into the
  * light list at upload: instances that carry them stay put (or re-upload). */
 RTXPT_API int rtxpt_b200_update_instance_transforms(rtxpt_ctx* ctx, const float* transforms3x4, uint32_t instanceCount, void* cudaStream);
+/* Rebuild of the 8-wide BVH on the GPU over the leaf triangles as they are now (after refits and skin updates), replacing the context's tree: what a DXR caller gets from a build
+ * without the update flag, where rtxpt_b200_update_instance_transforms is the update.  PLOC clustering over Morton-sorted triangles, the same 8-wide collapse, slot assignment and
+ * quantisation as the host builder.  The triangle set, gids, flags and opacity-mask slots stay; only the tree and the leaf order change.  The result is a function of the triangles alone
+ * (not of their current leaf order) and is the same in both libraries.  The work is enqueued on the stream, and the call waits for that stream after every clustering iteration
+ * and every tree level (to read back a count of a few bytes) and once at the end: it returns with the new tree in place.  Scratch memory is owned by the context and only grows
+ * (a few hundred bytes per triangle).  RTXPT_ERR_NO_SCENE before an upload; an empty scene is a no-op; RTXPT_ERR_UNSUPPORTED when the tree would be deeper than 32 levels (the
+ * traversal stack); on any error the previous tree stays.  Work that reads the tree must be ordered with this call on the stream, as with the refit. */
+RTXPT_API int rtxpt_b200_rebuild_bvh(rtxpt_ctx* ctx, void* cudaStream);
 /* Skinned meshes (Donut's skinning pass, External/Donut/shaders/skinning_cs.hlsl, which RTXPT runs before its BLAS updates, Sample.cpp:1170-1198): register a geometry's bind pose once
  * (vertex order = the geometry's vertex buffer; normals / tangents snorm8 x 4 as in the vertex buffer, may be NULL; four uint16 joint indices and four float weights per vertex), then per
  * frame hand the joint matrices (row-major 4x4, row vector x matrix, as Donut's t_JointMatrices): the vertices are blended on the stream and the path tracer's per-triangle shade
@@ -688,6 +696,9 @@ RTXPT_API const char* rtxpt_b200_load_hdr_image_error(void);
  * expected node visits / triangle tests of a random ray that hits the root box.  Used to judge builder changes without a GPU. */
 typedef struct RtxptBvhStats { uint32_t nodeCount, triangleReferenceCount, leafCount, maxDepth; float expectedNodeVisits, expectedTriangleTests, buildSeconds, _pad; } RtxptBvhStats;
 RTXPT_API int rtxpt_b200_debug_bvh_stats(const float* triangleVertices, uint32_t triangleCount, RtxptBvhStats* outStats);
+/* The same statistics of the context's tree as it is now (after upload, refit or rebuild), over the root's current box; buildSeconds is the last build: the host build at upload or
+ * the device rebuild (CUDA events).  Synchronises the context's stream and reads the nodes back. */
+RTXPT_API int rtxpt_b200_get_bvh_stats(rtxpt_ctx* ctx, RtxptBvhStats* outStats);
 
 /* StandardBSDF evaluated on the device for `count` records of 36 floats in / 16 floats out; see tests/test_bsdf_parity.py. */
 RTXPT_API int rtxpt_b200_debug_bsdf(rtxpt_ctx* ctx, const float* in, uint32_t count, float* out);

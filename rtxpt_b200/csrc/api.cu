@@ -9,6 +9,8 @@
 #include "neeat_host.h"
 #include "envbake.cuh"
 #include "refit.cuh"
+#include "bvh_build.cuh"
+#include "scan.cuh"
 #include "tonemap.cuh"
 #include "skinning.cuh"
 #include "lights_bake.h"
@@ -121,6 +123,11 @@ struct rtxpt_ctx
                   DeviceArray<float> positions, weights, outPositions, jointMatrices; DeviceArray<uint32_t> normals, tangents, outNormals, outTangents; DeviceArray<unsigned short> jointIndices; };
     std::vector<std::unique_ptr<Skin>> skins;
     uint32_t bvhNodeCount = 0, bvhTriCount = 0; float bvhBuildSeconds = 0;
+    float bvhRootBox[6] = {};           // exact box of the root as last built (the host build's scene bounds, or the device rebuild's root box): the SAH statistics' reference area
+    // device rebuild (bvh_build.cuh): scratch grown to the largest scene rebuilt, never shrunk; the new tree is built into `nodes` / `outTris` and swapped in on success
+    struct BvhScratch { DeviceArray<float4> tris, outTris; DeviceArray<uint4> nodes; DeviceArray<float> nodeBox, box2; DeviceArray<unsigned long long> keys[2], hist, flags, scanBlocks, misc;
+                        DeviceArray<uint32_t> vals[2], count2, clusters[2], nn, nodeRoot, cenBounds; DeviceArray<uint2> child2; } bvhScratch;
+    Event evBvhStart, evBvhStop;
     std::vector<RtxptSubInstanceData> hSubInstances; uint32_t materialCount = 0;
     LightBakeState lightState;
     DeviceArray<LightInfo> dLights; DeviceArray<uint32_t> dProxyCounters, dProxyIndices, dEnvLookup; DeviceArray<uint4> dLightsEx;
@@ -458,6 +465,7 @@ extern "C" RTXPT_API int rtxpt_b200_upload_scene(rtxpt_ctx* c, const RtxptSceneD
     c->bvhBuildSeconds = float(bvh.buildSeconds);
     { const float dx = bvh.sceneHi[0] - bvh.sceneLo[0], dy = bvh.sceneHi[1] - bvh.sceneLo[1], dz = bvh.sceneHi[2] - bvh.sceneLo[2]; c->sceneDiagonal = tris.empty() ? 0.0f : sqrtf(dx * dx + dy * dy + dz * dz); }
     c->bvhNodeCount = uint32_t(bvh.nodes.size()); c->bvhTriCount = uint32_t(bvh.tris.size());
+    for (int a = 0; a < 3; a++) { c->bvhRootBox[a] = bvh.sceneLo[a]; c->bvhRootBox[3 + a] = bvh.sceneHi[a]; }
     cudaStream_t s = c->stream;
     CU(c->dBvhNodes.upload(reinterpret_cast<const uint4*>(bvh.nodes.data()), bvh.nodes.size() * 5, s));
     CU(c->dBvhTris.upload(reinterpret_cast<const float4*>(bvh.tris.data()), bvh.tris.size() * 3, s));
@@ -977,6 +985,68 @@ extern "C" RTXPT_API int rtxpt_b200_update_instance_transforms(rtxpt_ctx* c, con
     p.nodes = c->dBvhNodes.ptr; p.tris = c->dBvhTris.ptr; p.triShade = c->dTriShade.ptr; p.instances = c->dInstances.ptr; p.nodeBox = c->dNodeBox.ptr; p.nodeCount = c->bvhNodeCount; p.triCount = c->bvhTriCount;
     launchRefit(p, c->bvhLevelStart.data(), uint32_t(c->bvhLevelStart.size()) - 1, c->grid.smCount, s);
     CU(cudaGetLastError());
+    return RTXPT_OK;
+}
+
+// ---- device rebuild of the BVH over the current leaf triangles (bvh_build.cuh; what Sample::BuildTLAS / UpdateSkinnedBLASs ask of the driver every frame, Sample.cpp:1170-1240) ----
+extern "C" RTXPT_API int rtxpt_b200_rebuild_bvh(rtxpt_ctx* c, void* cudaStream)
+{
+    if (!c) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (!c->haveScene) return fail(RTXPT_ERR_NO_SCENE, "no scene uploaded");
+    const uint32_t n = c->bvhTriCount;
+    if (n == 0) return RTXPT_OK;
+    cudaSetDevice(c->device);
+    cudaStream_t s = pickStream(c, cudaStream);
+    rtxpt_ctx::BvhScratch& b = c->bvhScratch;
+    const uint32_t tiles = (n + bvhb::kRadixTile - 1) / bvhb::kRadixTile;
+    const size_t scanLen = std::max<size_t>(n, size_t(tiles) * 256), nodeCap = n;       // at most one wide node per BVH2 node with children (n - 1), or the root alone
+    bool grown = false;
+    auto grow = [&](auto& a, size_t count) -> cudaError_t {
+        if (a.count >= count) return cudaSuccess;
+        if (!grown) { grown = true; cudaError_t e = syncContext(c); if (e != cudaSuccess) return e; }
+        return a.alloc(count);
+    };
+    CU(grow(b.tris, size_t(n) * 3)); CU(grow(b.outTris, size_t(n) * 3)); CU(grow(b.nodes, nodeCap * 5)); CU(grow(b.nodeBox, nodeCap * 6)); CU(grow(b.box2, size_t(n) * 12));
+    for (int k = 0; k < 2; k++) { CU(grow(b.keys[k], n)); CU(grow(b.vals[k], n)); CU(grow(b.clusters[k], n)); }
+    CU(grow(b.hist, size_t(tiles) * 256)); CU(grow(b.flags, n)); CU(grow(b.scanBlocks, (scanLen + kScanBlock - 1) / kScanBlock)); CU(grow(b.misc, 2));
+    CU(grow(b.count2, size_t(n) * 2)); CU(grow(b.nn, n)); CU(grow(b.nodeRoot, nodeCap)); CU(grow(b.cenBounds, 6)); CU(grow(b.child2, n));
+    if (!c->evBvhStart) { CU(c->evBvhStart.create(cudaEventCreateWithFlags, cudaEventDefault)); CU(c->evBvhStop.create(cudaEventCreateWithFlags, cudaEventDefault)); }
+    bvhb::Params p{};
+    p.srcTris = c->dBvhTris.ptr; p.tris = b.tris.ptr; p.triCount = n; p.cenBounds = b.cenBounds.ptr; p.varying = b.misc.ptr + 1;
+    for (int k = 0; k < 2; k++) { p.keys[k] = b.keys[k].ptr; p.vals[k] = b.vals[k].ptr; p.clusters[k] = b.clusters[k].ptr; }
+    p.hist = b.hist.ptr; p.box2 = b.box2.ptr; p.child2 = b.child2.ptr; p.count2 = b.count2.ptr; p.nn = b.nn.ptr; p.flags = b.flags.ptr;
+    p.nodeRoot = b.nodeRoot.ptr; p.levelCounts = b.flags.ptr;          // the PLOC flags are dead once the clustering is done
+    p.nodes = b.nodes.ptr; p.outTris = b.outTris.ptr; p.nodeBox = b.nodeBox.ptr;
+    CU(cudaEventRecord(c->evBvhStart, s));
+    BvhBuildResult r;
+    CU(launchBvhBuild(p, BvhBuildScans{ b.scanBlocks.ptr, b.misc.ptr }, c->grid.smCount, s, r));
+    if (r.status == BvhBuildResult::kTooDeep) return fail(RTXPT_ERR_UNSUPPORTED, "rebuilt BVH would be deeper than %u levels (traversal stack); the previous tree is kept", bvhb::kMaxDepth);
+    if (r.status != BvhBuildResult::kOk) return fail(RTXPT_ERR_INTERNAL, "BVH rebuild did not converge; the previous tree is kept");
+    CU(cudaEventRecord(c->evBvhStop, s)); CU(cudaEventSynchronize(c->evBvhStop));
+    float ms = 0; CU(cudaEventElapsedTime(&ms, c->evBvhStart, c->evBvhStop));
+    std::swap(c->dBvhNodes, b.nodes); std::swap(c->dBvhTris, b.outTris);
+    c->bvhNodeCount = r.nodeCount; c->bvhLevelStart = r.levelStart; c->dNodeBox = {};
+    for (int a = 0; a < 6; a++) c->bvhRootBox[a] = r.rootBox[a];
+    { const float dx = r.rootBox[3] - r.rootBox[0], dy = r.rootBox[4] - r.rootBox[1], dz = r.rootBox[5] - r.rootBox[2]; c->sceneDiagonal = sqrtf(dx * dx + dy * dy + dz * dz); }
+    c->bvhBuildSeconds = ms * 1e-3f;
+    return RTXPT_OK;
+}
+extern "C" RTXPT_API int rtxpt_b200_get_bvh_stats(rtxpt_ctx* c, RtxptBvhStats* out)
+{
+    if (!c || !out) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (!c->haveScene) return fail(RTXPT_ERR_NO_SCENE, "no scene uploaded");
+    cudaSetDevice(c->device);
+    memset(out, 0, sizeof(*out));
+    out->nodeCount = c->bvhNodeCount; out->triangleReferenceCount = c->bvhTriCount; out->maxDepth = uint32_t(c->bvhLevelStart.size()) - 1; out->buildSeconds = c->bvhBuildSeconds;
+    if (c->bvhTriCount == 0) return RTXPT_OK;
+    CU(syncContext(c));
+    std::vector<Bvh8Node> nodes(c->bvhNodeCount);
+    CU(cudaMemcpy(nodes.data(), c->dBvhNodes.ptr, nodes.size() * sizeof(Bvh8Node), cudaMemcpyDeviceToHost));
+    float root[6]; memcpy(root, c->bvhRootBox, 24);
+    if (c->dNodeBox.count >= 6) CU(cudaMemcpy(root, c->dNodeBox.ptr, 24, cudaMemcpyDeviceToHost));     // refitted since the last build: the root's exact box now
+    double visits = 0, tests = 0;
+    bvh8SahStats(nodes.data(), nodes.size(), root, root + 3, &visits, &tests, &out->leafCount);
+    out->expectedNodeVisits = float(visits); out->expectedTriangleTests = float(tests);
     return RTXPT_OK;
 }
 

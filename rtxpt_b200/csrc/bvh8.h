@@ -22,6 +22,7 @@
 #pragma once
 #include <stdint.h>
 #include <math.h>
+#include <string.h>
 #include <vector>
 
 namespace pt {
@@ -74,7 +75,55 @@ BVH8_HD void bvh8QuantizeChild(const float* nodeLo, const uint32_t* ebias, const
     }
 }
 
+// ---- octant slot assignment and node encoding, shared by the host builder (bvh_builder.cpp) and the device builder (bvh_build.cuh) ----
+// children (boxes in any order) -> slot of each: greedy maximum of dot(child centre - node centre, slot direction), first child / slot on ties
+BVH8_HD void bvh8AssignSlots(const float* nodeLo, const float* nodeHi, int nChild, const float (*childLo)[3], const float (*childHi)[3], int* childInSlot)
+{
+    float nc[3]; for (int a = 0; a < 3; a++) nc[a] = 0.5f * (nodeLo[a] + nodeHi[a]);
+    float cost[8][8];
+    for (int i = 0; i < nChild; i++)
+    {
+        float d[3]; for (int a = 0; a < 3; a++) d[a] = 0.5f * (childLo[i][a] + childHi[i][a]) - nc[a];
+        for (int s = 0; s < 8; s++) cost[i][s] = ((s & 4) ? d[0] : -d[0]) + ((s & 2) ? d[1] : -d[1]) + ((s & 1) ? d[2] : -d[2]);
+    }
+    int slotOf[8] = { 0, 0, 0, 0, 0, 0, 0, 0 }; bool slotUsed[8] = { false, false, false, false, false, false, false, false }; bool childDone[8] = { false, false, false, false, false, false, false, false };
+    for (int k = 0; k < nChild; k++)
+    {
+        float bestC = -3.0e38f; int bi = -1, bs = -1;
+        for (int i = 0; i < nChild; i++) if (!childDone[i]) for (int s = 0; s < 8; s++) if (!slotUsed[s] && cost[i][s] > bestC) { bestC = cost[i][s]; bi = i; bs = s; }
+        slotOf[bi] = bs; slotUsed[bs] = true; childDone[bi] = true;
+    }
+    for (int s = 0; s < 8; s++) childInSlot[s] = -1;
+    for (int i = 0; i < nChild; i++) childInSlot[slotOf[i]] = i;
+}
+// one 80-byte node from its box, the boxes of the used slots (meta[s] != 0), the slot metadata and the child / triangle bases: quantisation frame and conservative child boxes
+BVH8_HD void bvh8EncodeNode(const float* lo, const float* hi, const float (*slotLo)[3], const float (*slotHi)[3], const uint8_t* meta, uint32_t imask, uint32_t childBase, uint32_t triBase,
+                            uint32_t* w)
+{
+    uint32_t ebias[3];
+    for (int a = 0; a < 3; a++) ebias[a] = uint32_t(bvh8FrameExponent(double(hi[a]) - double(lo[a])) + 127);
+    uint8_t q[6][8];
+    for (int k = 0; k < 6; k++) for (int s = 0; s < 8; s++) q[k][s] = 0;
+    for (int s = 0; s < 8; s++)
+    {
+        if (meta[s] == 0) continue;
+        uint8_t ql[3], qh[3]; bvh8QuantizeChild(lo, ebias, slotLo[s], slotHi[s], ql, qh);
+        for (int a = 0; a < 3; a++) { q[a][s] = ql[a]; q[3 + a][s] = qh[a]; }
+    }
+    memcpy(&w[0], lo, 12);
+    w[3] = ebias[0] | (ebias[1] << 8) | (ebias[2] << 16) | (imask << 24);
+    w[4] = childBase; w[5] = triBase;
+    memcpy(&w[6], meta, 8);
+    memcpy(&w[8], q[0], 8);  memcpy(&w[10], q[1], 8);     // qlo.x | qlo.y
+    memcpy(&w[12], q[2], 8); memcpy(&w[14], q[3], 8);     // qlo.z | qhi.x
+    memcpy(&w[16], q[4], 8); memcpy(&w[18], q[5], 8);     // qhi.y | qhi.z
+}
+
 // Binned-SAH BVH2 -> greedy 8-wide collapse -> octant slot assignment -> quantisation.  Host only.
 void buildBvh8(const std::vector<BuildTriangle>& tris, Bvh8& out);
+
+// Surface-area-heuristic expectations of a tree (MacDonald & Booth) for a random ray that hits the root box [rootLo, rootHi]: a node is visited with probability
+// area(node) / area(root), using the quantised child boxes the traversal tests.  Host only; breadth-first node array (parents before children).
+void bvh8SahStats(const Bvh8Node* nodes, size_t nodeCount, const float* rootLo, const float* rootHi, double* expectedNodeVisits, double* expectedTriangleTests, uint32_t* leafCount);
 
 } // namespace pt

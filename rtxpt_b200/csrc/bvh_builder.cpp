@@ -171,35 +171,14 @@ void buildBvh8(const std::vector<BuildTriangle>& tris, Bvh8& out)
             uint32_t c = child[best];
             child[best] = N[c].left; child[nChild++] = N[c].right;
         }
-        // 2. octant slot assignment
+        // 2. octant slot assignment (bvh8.h)
         const Box& nb = N[rootIdx].box;
-        float nc[3]; for (int a = 0; a < 3; a++) nc[a] = 0.5f * (nb.lo[a] + nb.hi[a]);
-        float cost[8][8];
-        for (int i = 0; i < nChild; i++)
-        {
-            const Box& cb = N[child[i]].box;
-            float d[3]; for (int a = 0; a < 3; a++) d[a] = 0.5f * (cb.lo[a] + cb.hi[a]) - nc[a];
-            for (int s = 0; s < 8; s++) cost[i][s] = ((s & 4) ? d[0] : -d[0]) + ((s & 2) ? d[1] : -d[1]) + ((s & 1) ? d[2] : -d[2]);
-        }
-        int slotOf[8]; bool slotUsed[8] = { false, false, false, false, false, false, false, false }; bool childDone[8] = { false, false, false, false, false, false, false, false };
-        for (int k = 0; k < nChild; k++)
-        {
-            float bestC = -3.0e38f; int bi = -1, bs = -1;
-            for (int i = 0; i < nChild; i++) if (!childDone[i]) for (int s = 0; s < 8; s++) if (!slotUsed[s] && cost[i][s] > bestC) { bestC = cost[i][s]; bi = i; bs = s; }
-            slotOf[bi] = bs; slotUsed[bs] = true; childDone[bi] = true;
-        }
-        int childInSlot[8]; for (int s = 0; s < 8; s++) childInSlot[s] = -1;
-        for (int i = 0; i < nChild; i++) childInSlot[slotOf[i]] = i;
-        // 3. quantisation frame
-        uint32_t ebias[3];
-        for (int a = 0; a < 3; a++)
-        {
-            const int e = bvh8FrameExponent(double(nb.hi[a]) - double(nb.lo[a]));
-            ebias[a] = uint32_t(e + 127);
-        }
-        Bvh8Node node; memset(&node, 0, sizeof(node));
-        memcpy(&node.w[0], nb.lo, 12);
-        uint8_t meta[8] = { 0, 0, 0, 0, 0, 0, 0, 0 }; uint8_t q[6][8]; memset(q, 0, sizeof(q));
+        float childLo[8][3], childHi[8][3];
+        for (int i = 0; i < nChild; i++) for (int a = 0; a < 3; a++) { childLo[i][a] = N[child[i]].box.lo[a]; childHi[i][a] = N[child[i]].box.hi[a]; }
+        int childInSlot[8]; bvh8AssignSlots(nb.lo, nb.hi, nChild, childLo, childHi, childInSlot);
+        // 3. slot metadata, then the node's encoding (bvh8.h: quantisation frame and child boxes)
+        Bvh8Node node;
+        uint8_t meta[8] = { 0, 0, 0, 0, 0, 0, 0, 0 }; float slotLo[8][3], slotHi[8][3];
         uint32_t imask = 0;
         const uint32_t childBase = uint32_t(queue.size());
         const uint32_t triBase = uint32_t(out.tris.size());
@@ -209,7 +188,7 @@ void buildBvh8(const std::vector<BuildTriangle>& tris, Bvh8& out)
             int ci = childInSlot[s];
             if (ci < 0) continue;
             const Node2& c = N[child[ci]];
-            { uint8_t ql[3], qh[3]; bvh8QuantizeChild(nb.lo, ebias, c.box.lo, c.box.hi, ql, qh); for (int a = 0; a < 3; a++) { q[a][s] = ql[a]; q[3 + a][s] = qh[a]; } }
+            for (int a = 0; a < 3; a++) { slotLo[s][a] = c.box.lo[a]; slotHi[s][a] = c.box.hi[a]; }
             if (c.count == 0)
             {
                 imask |= 1u << s;
@@ -230,23 +209,44 @@ void buildBvh8(const std::vector<BuildTriangle>& tris, Bvh8& out)
                 triOffset += c.count;
             }
         }
-        node.w[3] = ebias[0] | (ebias[1] << 8) | (ebias[2] << 16) | (imask << 24);
-        node.w[4] = childBase; node.w[5] = triBase;
-        memcpy(&node.w[6], meta, 8);
-        memcpy(&node.w[8], q[0], 8);  memcpy(&node.w[10], q[1], 8);     // qlo.x | qlo.y
-        memcpy(&node.w[12], q[2], 8); memcpy(&node.w[14], q[3], 8);     // qlo.z | qhi.x
-        memcpy(&node.w[16], q[4], 8); memcpy(&node.w[18], q[5], 8);     // qhi.y | qhi.z
+        bvh8EncodeNode(nb.lo, nb.hi, slotLo, slotHi, meta, imask, childBase, triBase, node.w);
         out.nodes.push_back(node);
     }
     out.levelStart.push_back(uint32_t(out.nodes.size()));
     out.buildSeconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 
+void bvh8SahStats(const Bvh8Node* nodes, size_t nodeCount, const float* rootLo, const float* rootHi, double* expectedNodeVisits, double* expectedTriangleTests, uint32_t* leafCount)
+{
+    auto boxArea = [](const double* lo, const double* hi) { const double dx = hi[0] - lo[0], dy = hi[1] - lo[1], dz = hi[2] - lo[2]; return 2.0 * (dx * dy + dy * dz + dz * dx); };
+    double rLo[3], rHi[3]; for (int a = 0; a < 3; a++) { rLo[a] = rootLo[a]; rHi[a] = rootHi[a]; }
+    const double rootArea = std::max(boxArea(rLo, rHi), 1e-30);
+    // probability of visiting node i: carried down from the parent (quantised child box area / root area); breadth-first layout = parents first
+    std::vector<double> visitP(nodeCount, 0.0); if (nodeCount) visitP[0] = 1.0;
+    double nodeVisits = 0, triTests = 0, leaves = 0;
+    for (size_t ni = 0; ni < nodeCount; ni++)
+    {
+        const Bvh8Node& n = nodes[ni];
+        nodeVisits += visitP[ni];
+        float p[3]; memcpy(p, &n.w[0], 12);
+        const uint32_t e[3] = { n.w[3] & 0xFF, (n.w[3] >> 8) & 0xFF, (n.w[3] >> 16) & 0xFF }, imask = n.w[3] >> 24, childBase = n.w[4];
+        const uint8_t* meta = reinterpret_cast<const uint8_t*>(&n.w[6]); const uint8_t* q = reinterpret_cast<const uint8_t*>(&n.w[8]);
+        for (int s = 0; s < 8; s++)
+        {
+            if (meta[s] == 0) continue;
+            double lo[3], hi[3];
+            for (int a = 0; a < 3; a++) { const double sc = std::ldexp(1.0, int(e[a]) - 127); lo[a] = p[a] + q[a * 8 + s] * sc; hi[a] = p[a] + q[(3 + a) * 8 + s] * sc; }
+            const double pr = std::min(1.0, boxArea(lo, hi) / rootArea);
+            if (imask & (1u << s)) visitP[childBase + __builtin_popcount(imask & ((1u << s) - 1u))] = pr;
+            else { const int cnt = __builtin_popcount(uint32_t(meta[s] >> 5)); triTests += pr * cnt; leaves += 1; }
+        }
+    }
+    *expectedNodeVisits = nodeVisits; *expectedTriangleTests = triTests; *leafCount = uint32_t(leaves);
+}
+
 } // namespace pt
 
-// ---- inspection hook (host only): surface-area-heuristic statistics of the tree built over a triangle soup -----------------------------------------------
-// Expected work of a random ray that hits the root box (MacDonald & Booth): a node is visited with probability area(node) / area(root);
-// the child boxes used are the quantised ones the traversal tests.
+// ---- inspection hook (host only): surface-area-heuristic statistics of the tree built over a triangle soup (bvh8SahStats) -----------------------------------------------
 #include "../../include/rtxpt_b200.h"
 extern "C" RTXPT_API int rtxpt_b200_debug_bvh_stats(const float* triangleVertices, uint32_t triangleCount, RtxptBvhStats* out)
 {
@@ -262,30 +262,9 @@ extern "C" RTXPT_API int rtxpt_b200_debug_bvh_stats(const float* triangleVertice
     memset(out, 0, sizeof(*out));
     out->nodeCount = uint32_t(bvh.nodes.size()); out->triangleReferenceCount = uint32_t(bvh.tris.size()); out->buildSeconds = float(bvh.buildSeconds); out->maxDepth = bvh.maxDepth;
     if (triangleCount == 0) return RTXPT_OK;
-    auto boxArea = [](const double* lo, const double* hi) { const double dx = hi[0] - lo[0], dy = hi[1] - lo[1], dz = hi[2] - lo[2]; return 2.0 * (dx * dy + dy * dz + dz * dx); };
-    double rootLo[3], rootHi[3]; for (int a = 0; a < 3; a++) { rootLo[a] = bvh.sceneLo[a]; rootHi[a] = bvh.sceneHi[a]; }
-    const double rootArea = std::max(boxArea(rootLo, rootHi), 1e-30);
-    // probability of visiting node i: carried down from the parent (quantised child box area / root area); breadth-first layout = parents first
-    std::vector<double> visitP(bvh.nodes.size(), 0.0); visitP[0] = 1.0;
-    double nodeVisits = 0, triTests = 0, leafCount = 0;
-    for (size_t ni = 0; ni < bvh.nodes.size(); ni++)
-    {
-        const Bvh8Node& n = bvh.nodes[ni];
-        nodeVisits += visitP[ni];
-        float p[3]; memcpy(p, &n.w[0], 12);
-        const uint32_t e[3] = { n.w[3] & 0xFF, (n.w[3] >> 8) & 0xFF, (n.w[3] >> 16) & 0xFF }, imask = n.w[3] >> 24, childBase = n.w[4];
-        const uint8_t* meta = reinterpret_cast<const uint8_t*>(&n.w[6]); const uint8_t* q = reinterpret_cast<const uint8_t*>(&n.w[8]);
-        for (int s = 0; s < 8; s++)
-        {
-            if (meta[s] == 0) continue;
-            double lo[3], hi[3];
-            for (int a = 0; a < 3; a++) { const double sc = std::ldexp(1.0, int(e[a]) - 127); lo[a] = p[a] + q[a * 8 + s] * sc; hi[a] = p[a] + q[(3 + a) * 8 + s] * sc; }
-            const double pr = std::min(1.0, boxArea(lo, hi) / rootArea);
-            if (imask & (1u << s)) visitP[childBase + __builtin_popcount(imask & ((1u << s) - 1u))] = pr;
-            else { const int cnt = __builtin_popcount(uint32_t(meta[s] >> 5)); triTests += pr * cnt; leafCount += 1; }
-        }
-    }
-    out->expectedNodeVisits = float(nodeVisits); out->expectedTriangleTests = float(triTests); out->leafCount = uint32_t(leafCount);
+    double nodeVisits = 0, triTests = 0;
+    bvh8SahStats(bvh.nodes.data(), bvh.nodes.size(), bvh.sceneLo, bvh.sceneHi, &nodeVisits, &triTests, &out->leafCount);
+    out->expectedNodeVisits = float(nodeVisits); out->expectedTriangleTests = float(triTests);
     return RTXPT_OK;
 }
 

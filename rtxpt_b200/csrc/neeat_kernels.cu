@@ -7,6 +7,7 @@
 // bodies pass tests/test_neeat_port.py on the CPU.
 #include "neeat.cuh"
 #include "kernels.h"
+#include "scan.cuh"
 
 namespace pt { namespace neeat {
 
@@ -43,28 +44,7 @@ __global__ void __launch_bounds__(256) k_na_proxy_counts(const __grid_constant__
     if (i < p.lightCount) p.proxyCounters[i] = proxyCountOfLight(p, i);
 }
 
-// ---- exclusive scan of proxyCounters[0 .. lightCount) into proxyOffsets[0 .. lightCount], total into *samplingProxyCount --------------------------------------------------------
-constexpr uint kScanBlock = 1024;
-__device__ __forceinline__ uint blockExclusiveScan(uint v, uint* warpSums /* 32 */, uint& blockTotal)
-{
-    const uint lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint inc = v;
-    #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint n = __shfl_up_sync(0xFFFFFFFFu, inc, d); if (lane >= uint(d)) inc += n; }
-    if (lane == 31) warpSums[warp] = inc;
-    __syncthreads();
-    if (warp == 0)
-    {
-        uint w = warpSums[lane], winc = w;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint n = __shfl_up_sync(0xFFFFFFFFu, winc, d); if (lane >= uint(d)) winc += n; }
-        warpSums[lane] = winc - w;                      // exclusive warp offsets
-        if (lane == 31) warpSums[32] = winc;            // block total
-    }
-    __syncthreads();
-    blockTotal = warpSums[32];
-    return inc - v + warpSums[warp];
-}
+// ---- exclusive scan of proxyCounters[0 .. lightCount) into proxyOffsets[0 .. lightCount], total into *samplingProxyCount (blockExclusiveScan: scan.cuh) ----------------------------
 __global__ void __launch_bounds__(kScanBlock) k_na_scan_reduce(const __grid_constant__ Params p, uint* blockSums)
 {
     __shared__ uint ws[33];

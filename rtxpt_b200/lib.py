@@ -58,6 +58,8 @@ _SIGNATURES = {
     "rtxpt_b200_tone_map": [C.c_void_p, C.POINTER(S.ToneMappingParams), C.c_int, C.c_void_p],
     "rtxpt_b200_tone_map_average_luminance": [C.c_void_p, C.POINTER(C.c_float)],
     "rtxpt_b200_update_instance_transforms": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p],
+    "rtxpt_b200_rebuild_bvh": [C.c_void_p, C.c_void_p],
+    "rtxpt_b200_get_bvh_stats": [C.c_void_p, C.POINTER(S.BvhStats)],
     "rtxpt_b200_bake_env_map": [C.c_void_p, C.POINTER(S.EnvBakeDesc), C.c_void_p, C.c_size_t],
     "rtxpt_b200_neeat_update_begin": [C.c_void_p, C.c_void_p],
     "rtxpt_b200_neeat_update_end": [C.c_void_p, C.c_void_p],
@@ -395,6 +397,15 @@ class Context:
         """transforms: instanceCount x 3 x 4 float32 (row-major): re-transforms the leaf triangles and refits the BVH on the stream."""
         t = np.ascontiguousarray(transforms, np.float32).reshape(-1, 12)
         _check(self.L.rtxpt_b200_update_instance_transforms(self.h, t.ctypes.data, len(t), stream), self.L)
+
+    def rebuild_bvh(self, stream=None):
+        """Rebuilds the BVH on the GPU over the leaf triangles as they are now (after update_instance_transforms / skin_update) and replaces the context's tree; returns with it in place."""
+        _check(self.L.rtxpt_b200_rebuild_bvh(self.h, stream), self.L)
+
+    def bvh_stats(self):
+        """SAH statistics (structs.BvhStats) of the context's tree as it is now; buildSeconds: the last build (host at upload, or the device rebuild)."""
+        st = S.BvhStats(); _check(self.L.rtxpt_b200_get_bvh_stats(self.h, C.byref(st)), self.L)
+        return st
 
     def bake_env_map(self, cube_dim, source=None, source_type=None, scale_color=(1.0, 1.0, 1.0), lights=()):
         """EnvMapBaker on the GPU.  source: HxWx4 float32 equirectangular image or 6xNxNx4 cube (None = lights only); lights: (colour rgb, intensity W/sr, incoming direction,
