@@ -441,7 +441,9 @@ RTXPT_API int rtxpt_b200_skin_register(rtxpt_ctx* ctx, const RtxptSkinDesc* desc
 RTXPT_API int rtxpt_b200_skin_update(rtxpt_ctx* ctx, uint32_t skinId, const float* jointMatrices4x4, uint32_t numJoints, void* cudaStream);
 /* tests / debugging: what = 0 BVH nodes (80 B each), 1 leaf triangles (48 B), 2 per-triangle shade records (96 B, by global triangle id),
  * 3 previous-position records (36 B), 4 instance table (RtxptInstanceData), 5 BVH level starts (uint32, levelCount + 1),
- * 6 exact node boxes of the last refit (6 floats per node; empty before the first refit).  dst == NULL returns the size in *outBytes; synchronises the context's stream. */
+ * 6 exact node boxes of the last refit (6 floats per node; empty before the first refit), 7 the environment cube's MIP chain (the layout rtxpt_b200_bake_env_map returns; empty
+ * without a cube), 8 the 1024^2 radiance / importance MIP chain (RGBA32F, MIPs back to back), 9 the environment lookup map (1024^2 uint32 light indices; empty while the environment
+ * is disabled).  dst == NULL returns the size in *outBytes; synchronises the context's stream. */
 RTXPT_API int rtxpt_b200_debug_scene_readback(rtxpt_ctx* ctx, int what, void* dst, size_t dstBytes, size_t* outBytes);
 /* host-only inspection of the builder: the compressed BVH over a triangle soup (nodes 80 B, leaf triangles 48 B with gid = soup index, level ranges); call with NULL outputs for sizes */
 RTXPT_API int rtxpt_b200_debug_build_bvh(const float* triangleVertices, uint32_t triangleCount, void* outNodes, void* outTris, uint32_t* outLevelStart,
@@ -464,6 +466,18 @@ typedef struct RtxptEnvBakeDesc {
 RTXPT_API uint32_t rtxpt_b200_env_bake_mip_count(uint32_t cubeDim);
 RTXPT_API size_t   rtxpt_b200_env_bake_floats(uint32_t cubeDim);          /* all MIPs back to back */
 RTXPT_API int      rtxpt_b200_bake_env_map(rtxpt_ctx* ctx, const RtxptEnvBakeDesc* desc, float* outAllMips, size_t outFloats);
+/* Re-bakes the environment of a live context on the GPU (EnvMapBaker::Update when it reports contentsChanged: the sun moved, the environment map was switched): the bake goes
+ * straight into the cube the path tracer samples, the 1024^2 radiance / importance map (EnvMapImportanceSamplingBaker) is rebuilt from it on the GPU, and the environment's
+ * quad-tree lights, lookup map, weights and proxy table are re-baked on the host from that map.  Only the importance map (~22 MB) crosses to the host; nothing else of the scene is
+ * touched (BVH, skins, instance table, emissive triangles stay as they are).  Validation is that of rtxpt_b200_bake_env_map, except that source == NULL with sourceType 1 or 2
+ * re-bakes from the source the context kept from its last update (same type and size, else RTXPT_ERR_INVALID_ARGUMENT).  cubeDim may differ from the uploaded cube; a scene
+ * uploaded without a cube gains one.  On failure the previous cube, importance map and light list stay.  Like rtxpt_b200_update_lights: waits for the context's work in flight,
+ * returns with the new light list on the device when constants are set (otherwise rtxpt_b200_set_constants uploads it), and NEE-AT's next update_begin maps last frame's feedback
+ * onto the new environment nodes.  The importance map of an update and of an upload are built by the same arithmetic on GPU and host, but the GPU's cos / sin round differently
+ * from the C library's in a small share of taps, so the two maps differ in a small share of texels. */
+RTXPT_API int      rtxpt_b200_update_env_map(rtxpt_ctx* ctx, const RtxptEnvBakeDesc* desc, void* cudaStream);
+/* event times of the last rtxpt_b200_update_env_map in ms: bake, importance map, copy into the cube array, read-back + host light bake + upload */
+RTXPT_API int      rtxpt_b200_last_env_update_ms(rtxpt_ctx* ctx, float* outMs4);
 
 /* ---- NEE-AT temporal feedback (SURVEY §8f row 1; replaces the feedback half of Rtxpt/Lighting/LightsBaker: UpdateBegin's ProcessFeedbackHistoryPreFilter / P0 + usage-weighted
  * ComputeProxyCounts, UpdateEnd's P1a / P1b / P2 / P3 / ClearFeedbackHistory, LightsBaker.cpp:1203-1225, :1331-1418).  Active with NEEType == 2 && NEEATFeedback != 0: NEE then draws
@@ -478,7 +492,7 @@ RTXPT_API int rtxpt_b200_neeat_update_end(rtxpt_ctx* ctx, void* cudaStream);
  * end keep their identity by position in the array; the library re-bakes its light list (environment nodes, analytic lights, emissive triangles) as LightsBaker::UpdateBegin does
  * every frame.  With NEE-AT feedback active the reservoirs and tile samplers of the last frame follow the lights through the past -> current index tables of the reference
  * (LightsBaker.hlsl u_historyRemapPastToCurrent / CurrentToPast: environment nodes through the importance-map lookups, triangles by block offset); a removed light's feedback is
- * dropped.  Call before rtxpt_b200_neeat_update_begin of the frame.  Emissive geometry and the environment cube stay those of the upload. */
+ * dropped.  Call before rtxpt_b200_neeat_update_begin of the frame.  Emissive geometry stays that of the upload; the environment changes through rtxpt_b200_update_env_map. */
 RTXPT_API int rtxpt_b200_update_lights(rtxpt_ctx* ctx, const RtxptLightDesc* lights, uint32_t lightCount);
 RTXPT_API int rtxpt_b200_neeat_reset(rtxpt_ctx* ctx);                 /* LightsBaker::BakeSettings::ResetFeedback: drop all feedback state */
 /* tests / debugging: what = 0,1 feedback weight / candidate; 2,3 processed; 4,5 half-resolution blend; 6 tile lists; 7 proxy counters; 8 control words; 11 proxy table */

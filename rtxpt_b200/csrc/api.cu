@@ -112,6 +112,10 @@ struct rtxpt_ctx
     std::vector<DeviceArray<uint8_t>> bufferAllocs; DeviceArray<const uint8_t*> dBufferTable;
     std::vector<DeviceTexture> textures; DeviceArray<cudaTextureObject_t> dTextureTable;
     DeviceTexture envCube; uint32_t envFaceSize = 0, envMipLevels = 0;
+    // rtxpt_b200_update_env_map: the bake's linear MIP chain and the importance map's, grown to the largest cube baked and never shrunk; the source of the last update, kept so
+    // that the next update can re-bake from it; event times of the last update (bake, importance map, copy into the cube, readback + light bake + upload)
+    DeviceArray<float> envBakeScratch, envImportanceScratch, envSource; uint32_t envSourceType = 0, envSourceWidth = 0, envSourceHeight = 0;
+    Event evEnv[5]; float envUpdateMs[4] = {};
     DeviceArray<uint4> dBvhNodes; DeviceArray<float4> dBvhTris; DeviceArray<uint4> dTriInfo, dTriShade, dOpacityMasks;
     uint32_t opacityMaskTriangles = 0; uint64_t opacityMaskStates[3] = { 0, 0, 0 }; float opacityMaskBakeSeconds = 0;
     std::vector<RtxptInstanceData> hInstances; std::vector<uint32_t> bvhLevelStart; DeviceArray<float> dNodeBox;      // rigid-instance animation (refit.cuh)
@@ -315,11 +319,24 @@ static int createTexture2D(const RtxptTextureDesc& d, DeviceTexture& out)
     return RTXPT_OK;
 }
 
+// the layered, mipmapped float4 array of the environment cube and the texture object the kernels sample it through (filled by the caller)
+static int allocEnvCube(uint32_t faceSize, uint32_t mipLevels, DeviceTexture& out)
+{
+    cudaChannelFormatDesc fmt = cudaCreateChannelDesc<float4>();
+    CU(out.array.create(cudaMallocMipmappedArray, &fmt, make_cudaExtent(faceSize, faceSize, 6), mipLevels, cudaArrayLayered));
+    cudaResourceDesc res{}; res.resType = cudaResourceTypeMipmappedArray; res.res.mipmap.mipmap = out.array;
+    cudaTextureDesc td{};
+    td.addressMode[0] = td.addressMode[1] = cudaAddressModeClamp; td.addressMode[2] = cudaAddressModeClamp;
+    td.filterMode = cudaFilterModeLinear; td.mipmapFilterMode = cudaFilterModePoint; td.readMode = cudaReadModeElementType;
+    td.normalizedCoords = 1; td.maxAnisotropy = 1; td.maxMipmapLevelClamp = float(mipLevels - 1);
+    CU(out.object.create(cudaCreateTextureObject, &res, &td, nullptr));
+    return RTXPT_OK;
+}
+
 static int createEnvCube(const RtxptEnvCubeDesc& d, DeviceTexture& out)
 {
     if (d.mipLevels == 0 || d.mipLevels > RTXPT_MAX_MIPS) return fail(RTXPT_ERR_INVALID_ARGUMENT, "bad env cube description");
-    cudaChannelFormatDesc fmt = cudaCreateChannelDesc<float4>();
-    CU(out.array.create(cudaMallocMipmappedArray, &fmt, make_cudaExtent(d.faceSize, d.faceSize, 6), d.mipLevels, cudaArrayLayered));
+    int rc = allocEnvCube(d.faceSize, d.mipLevels, out); if (rc != RTXPT_OK) return rc;
     for (uint32_t m = 0; m < d.mipLevels; m++)
     {
         cudaArray_t level; CU(cudaGetMipmappedArrayLevel(&level, out.array, m));
@@ -333,12 +350,6 @@ static int createEnvCube(const RtxptEnvCubeDesc& d, DeviceTexture& out)
             CU(cudaMemcpy3D(&cp));
         }
     }
-    cudaResourceDesc res{}; res.resType = cudaResourceTypeMipmappedArray; res.res.mipmap.mipmap = out.array;
-    cudaTextureDesc td{};
-    td.addressMode[0] = td.addressMode[1] = cudaAddressModeClamp; td.addressMode[2] = cudaAddressModeClamp;
-    td.filterMode = cudaFilterModeLinear; td.mipmapFilterMode = cudaFilterModePoint; td.readMode = cudaReadModeElementType;
-    td.normalizedCoords = 1; td.maxAnisotropy = 1; td.maxMipmapLevelClamp = float(d.mipLevels - 1);
-    CU(out.object.create(cudaCreateTextureObject, &res, &td, nullptr));
     return RTXPT_OK;
 }
 
@@ -1133,42 +1144,140 @@ extern "C" RTXPT_API int rtxpt_b200_debug_scene_readback(rtxpt_ctx* c, int what,
     case 4: src = c->dInstances.ptr; bytes = c->hInstances.size() * sizeof(RtxptInstanceData); break;
     case 5: src = c->bvhLevelStart.data(); bytes = c->bvhLevelStart.size() * 4; host = true; break;
     case 6: src = c->dNodeBox.ptr; bytes = c->dNodeBox.count * 4; break;
+    case 7: if (c->envCube.array) for (uint32_t m = 0; m < c->envMipLevels; m++) bytes += size_t(6) * (c->envFaceSize >> m) * (c->envFaceSize >> m) * 16; break;
+    case 8: for (const std::vector<float>& mip : c->lightState.envRadianceMips) bytes += mip.size() * 4; break;
+    case 9: src = c->dEnvLookup.ptr; bytes = c->dEnvLookup.count * 4; break;
     default: return fail(RTXPT_ERR_INVALID_ARGUMENT, "unknown scene buffer %d", what);
     }
     *outBytes = bytes;
     if (!dst || bytes == 0) return RTXPT_OK;
     if (dstBytes < bytes) return fail(RTXPT_ERR_INVALID_ARGUMENT, "destination too small (%zu < %zu)", dstBytes, bytes);
-    if (host) memcpy(dst, src, bytes); else CU(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
+    if (what == 7)
+    {   // the cube array, MIP by MIP, six faces back to back (the layout rtxpt_b200_bake_env_map returns)
+        size_t off = 0;
+        for (uint32_t m = 0; m < c->envMipLevels; m++)
+        {
+            const uint32_t n = c->envFaceSize >> m;
+            cudaArray_t level; CU(cudaGetMipmappedArrayLevel(&level, c->envCube.array, m));
+            cudaMemcpy3DParms cp{};
+            cp.srcArray = level; cp.dstPtr = make_cudaPitchedPtr(static_cast<uint8_t*>(dst) + off, size_t(n) * 16, n, n); cp.extent = make_cudaExtent(n, n, 6); cp.kind = cudaMemcpyDeviceToHost;
+            CU(cudaMemcpy3D(&cp));
+            off += size_t(6) * n * n * 16;
+        }
+    }
+    else if (what == 8) { size_t off = 0; for (const std::vector<float>& mip : c->lightState.envRadianceMips) { memcpy(static_cast<uint8_t*>(dst) + off, mip.data(), mip.size() * 4); off += mip.size() * 4; } }
+    else if (host) memcpy(dst, src, bytes); else CU(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
     return RTXPT_OK;
 }
 
 // ---- environment-map baking (SURVEY §8f row 3) ---------------------------------------------------------------------------------------------------------------------
 extern "C" RTXPT_API uint32_t rtxpt_b200_env_bake_mip_count(uint32_t cubeDim) { uint32_t l = 0; while ((cubeDim >> l) > 0) l++; return l; }
 extern "C" RTXPT_API size_t rtxpt_b200_env_bake_floats(uint32_t cubeDim) { size_t n = 0; for (uint32_t m = 0; (cubeDim >> m) > 0; m++) n += size_t(6) * (cubeDim >> m) * (cubeDim >> m) * 4; return n; }
+// what rtxpt_b200_bake_env_map and rtxpt_b200_update_env_map accept; `sourceMayBeKept`: a cube or equirectangular source may come without pixels (the context's kept source)
+static int checkEnvBakeDesc(const RtxptEnvBakeDesc* d, bool sourceMayBeKept)
+{
+    if (d->cubeDim < 2 || d->cubeDim > 4096 || (d->cubeDim & (d->cubeDim - 1))) return fail(RTXPT_ERR_INVALID_ARGUMENT, "cubeDim must be a power of two in 2..4096");
+    if (d->directionalLightCount > 16) return fail(RTXPT_ERR_INVALID_ARGUMENT, "at most 16 directional lights (EMB_MAXDIRLIGHTS)");
+    if (d->sourceType > 2 || (d->sourceType != 0 && ((!d->source && !sourceMayBeKept) || d->sourceWidth == 0 || (d->sourceType == 1 && d->sourceHeight == 0)))) return fail(RTXPT_ERR_INVALID_ARGUMENT, "bad source description");
+    return RTXPT_OK;
+}
+static size_t envSourceFloats(const RtxptEnvBakeDesc* d) { return d->sourceType == 1 ? size_t(d->sourceWidth) * d->sourceHeight * 4 : (d->sourceType == 2 ? size_t(6) * d->sourceWidth * d->sourceWidth * 4 : 0); }
+// the bake of `d` from `source` (device, NULL without one) into `mips`: all MIPs back to back, rtxpt_b200_env_bake_floats(cubeDim) floats
+static envbake::Params envBakeParams(const RtxptEnvBakeDesc* d, const float* source, float* mips)
+{
+    envbake::Params p{};
+    p.cubeDim = d->cubeDim; p.sourceType = d->sourceType; p.sourceWidth = d->sourceWidth; p.sourceHeight = d->sourceHeight; p.source = source;
+    memcpy(p.scaleColor, d->scaleColor, 12); p.lightCount = d->directionalLightCount;
+    for (uint32_t i = 0; i < d->directionalLightCount; i++) { memcpy(p.lights[i].colorIntensity, d->lights[i].colorIntensity, 16); memcpy(p.lights[i].direction, d->lights[i].direction, 12); p.lights[i].angularSize = d->lights[i].angularSize; }
+    size_t off = 0; for (uint32_t m = 0; m < rtxpt_b200_env_bake_mip_count(d->cubeDim); m++) { p.mips[m] = mips + off; off += size_t(6) * (d->cubeDim >> m) * (d->cubeDim >> m) * 4; }
+    return p;
+}
 extern "C" RTXPT_API int rtxpt_b200_bake_env_map(rtxpt_ctx* c, const RtxptEnvBakeDesc* d, float* out, size_t outFloats)
 {
     if (!c || !d || !out) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
-    if (d->cubeDim < 2 || d->cubeDim > 4096 || (d->cubeDim & (d->cubeDim - 1))) return fail(RTXPT_ERR_INVALID_ARGUMENT, "cubeDim must be a power of two in 2..4096");
-    if (d->directionalLightCount > 16) return fail(RTXPT_ERR_INVALID_ARGUMENT, "at most 16 directional lights (EMB_MAXDIRLIGHTS)");
-    if (d->sourceType > 2 || (d->sourceType != 0 && (!d->source || d->sourceWidth == 0 || (d->sourceType == 1 && d->sourceHeight == 0)))) return fail(RTXPT_ERR_INVALID_ARGUMENT, "bad source description");
+    int rc = checkEnvBakeDesc(d, false); if (rc != RTXPT_OK) return rc;
     const size_t total = rtxpt_b200_env_bake_floats(d->cubeDim);
     if (outFloats < total) return fail(RTXPT_ERR_INVALID_ARGUMENT, "output too small (%zu < %zu floats)", outFloats, total);
     cudaSetDevice(c->device);
     cudaStream_t s = c->stream;
     const uint32_t levels = rtxpt_b200_env_bake_mip_count(d->cubeDim);
     DeviceArray<float> src, dst;
-    const size_t srcFloats = d->sourceType == 1 ? size_t(d->sourceWidth) * d->sourceHeight * 4 : (d->sourceType == 2 ? size_t(6) * d->sourceWidth * d->sourceWidth * 4 : 0);
+    const size_t srcFloats = envSourceFloats(d);
     if (srcFloats) CU(src.upload(d->source, srcFloats, s));
     CU(dst.alloc(total));
-    envbake::Params p{};
-    p.cubeDim = d->cubeDim; p.sourceType = d->sourceType; p.sourceWidth = d->sourceWidth; p.sourceHeight = d->sourceHeight; p.source = src.ptr;
-    memcpy(p.scaleColor, d->scaleColor, 12); p.lightCount = d->directionalLightCount;
-    for (uint32_t i = 0; i < d->directionalLightCount; i++) { memcpy(p.lights[i].colorIntensity, d->lights[i].colorIntensity, 16); memcpy(p.lights[i].direction, d->lights[i].direction, 12); p.lights[i].angularSize = d->lights[i].angularSize; }
-    size_t off = 0; for (uint32_t m = 0; m < levels; m++) { p.mips[m] = dst.ptr + off; off += size_t(6) * (d->cubeDim >> m) * (d->cubeDim >> m) * 4; }
-    launchEnvBake(p, levels, s);
+    launchEnvBake(envBakeParams(d, src.ptr, dst.ptr), levels, s);
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(out, dst.ptr, total * 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
+    return RTXPT_OK;
+}
+
+// EnvMapBaker::Update with contentsChanged, then EnvMapImportanceSamplingBaker and the environment passes of LightsBaker (Sample.cpp, UpdateLighting): the bake goes straight into
+// the cube the kernels sample, the importance map is built on the GPU from it, and the host light bake builds the quad-tree lights from that map
+extern "C" RTXPT_API int rtxpt_b200_update_env_map(rtxpt_ctx* c, const RtxptEnvBakeDesc* d, void* cudaStream)
+{
+    if (!c || !d) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (!c->haveScene) return fail(RTXPT_ERR_NO_SCENE, "no scene uploaded");
+    int rc = checkEnvBakeDesc(d, true); if (rc != RTXPT_OK) return rc;
+    const bool keptSource = d->sourceType != 0 && !d->source;
+    if (keptSource && (!c->envSource.ptr || c->envSourceType != d->sourceType || c->envSourceWidth != d->sourceWidth || (d->sourceType == 1 && c->envSourceHeight != d->sourceHeight)))
+        return fail(RTXPT_ERR_INVALID_ARGUMENT, "no kept source of type %u and size %ux%u to re-bake from", d->sourceType, d->sourceWidth, d->sourceType == 1 ? d->sourceHeight : d->sourceWidth);
+    cudaSetDevice(c->device);
+    CU(syncContext(c));
+    cudaStream_t s = pickStream(c, cudaStream);
+    const uint32_t dim = d->cubeDim, levels = rtxpt_b200_env_bake_mip_count(dim);
+    const size_t bakeFloats = rtxpt_b200_env_bake_floats(dim);
+    size_t importanceFloats = 0; for (uint32_t m = 0; m < envbake::kImportanceMips; m++) importanceFloats += size_t(envbake::kImportanceDim >> m) * (envbake::kImportanceDim >> m) * 4;
+    if (c->envBakeScratch.count < bakeFloats) CU(c->envBakeScratch.alloc(bakeFloats));
+    if (c->envImportanceScratch.count < importanceFloats) CU(c->envImportanceScratch.alloc(importanceFloats));
+    if (!c->evEnv[0]) for (Event& e : c->evEnv) CU(e.create(cudaEventCreateWithFlags, cudaEventDefault));
+    DeviceArray<float> fresh;         // a new source replaces the kept one once the update has succeeded
+    if (d->sourceType != 0 && !keptSource) CU(fresh.upload(d->source, envSourceFloats(d), s));
+    CU(cudaEventRecord(c->evEnv[0], s));
+    launchEnvBake(envBakeParams(d, d->sourceType == 0 ? nullptr : (keptSource ? c->envSource.ptr : fresh.ptr), c->envBakeScratch.ptr), levels, s);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->evEnv[1], s));
+    envbake::ImportanceParams ip{};
+    ip.cube = c->envBakeScratch.ptr; ip.faceSize = dim;
+    { size_t off = 0; for (uint32_t m = 0; m < envbake::kImportanceMips; m++) { ip.mips[m] = c->envImportanceScratch.ptr + off; off += size_t(envbake::kImportanceDim >> m) * (envbake::kImportanceDim >> m) * 4; } }
+    launchEnvImportance(ip, s);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->evEnv[2], s));
+    // the cube: a new array only when its size changes (the old one stays in place until the update succeeds), otherwise the bake is copied over the one the kernels sample
+    DeviceTexture grown;
+    const bool newCube = !c->envCube.array || c->envFaceSize != dim || c->envMipLevels != levels;
+    if (newCube) { rc = allocEnvCube(dim, levels, grown); if (rc != RTXPT_OK) return rc; }
+    {
+        size_t off = 0;
+        for (uint32_t m = 0; m < levels; m++)
+        {   // MIP m of the bake is already six faces back to back: one copy into the six layers
+            const uint32_t n = dim >> m;
+            cudaArray_t level; CU(cudaGetMipmappedArrayLevel(&level, newCube ? grown.array : c->envCube.array, m));
+            cudaMemcpy3DParms cp{};
+            cp.srcPtr = make_cudaPitchedPtr(c->envBakeScratch.ptr + off, size_t(n) * 16, n, n); cp.dstArray = level; cp.extent = make_cudaExtent(n, n, 6); cp.kind = cudaMemcpyDeviceToDevice;
+            CU(cudaMemcpy3DAsync(&cp, s));
+            off += size_t(6) * n * n * 4;
+        }
+    }
+    CU(cudaEventRecord(c->evEnv[3], s));
+    // hand-off to the host light bake: the importance chain (the quad-tree, lookup map, weights and proxy table stay LightBaker's)
+    std::vector<std::vector<float>> chain(envbake::kImportanceMips);
+    { size_t off = 0; for (uint32_t m = 0; m < envbake::kImportanceMips; m++) { chain[m].resize(size_t(envbake::kImportanceDim >> m) * (envbake::kImportanceDim >> m) * 4); CU(cudaMemcpyAsync(chain[m].data(), c->envImportanceScratch.ptr + off, chain[m].size() * 4, cudaMemcpyDeviceToHost, s)); off += chain[m].size(); } }
+    CU(cudaStreamSynchronize(s));
+    if (newCube) { c->envCube = std::move(grown); c->envFaceSize = dim; c->envMipLevels = levels; }
+    if (fresh.ptr) { c->envSource = std::move(fresh); c->envSourceType = d->sourceType; c->envSourceWidth = d->sourceWidth; c->envSourceHeight = d->sourceType == 1 ? d->sourceHeight : d->sourceWidth; }
+    LightBakeState& st = c->lightState;
+    st.hasEnvCube = true; st.envMipCount = envbake::kImportanceMips; st.envRadianceMips = std::move(chain);
+    c->lightsDirty = true;
+    if (c->haveConstants) { rc = uploadLights(c); if (rc != RTXPT_OK) return rc; }
+    CU(cudaEventRecord(c->evEnv[4], s)); CU(cudaEventSynchronize(c->evEnv[4]));
+    for (int k = 0; k < 4; k++) CU(cudaEventElapsedTime(&c->envUpdateMs[k], c->evEnv[k], c->evEnv[k + 1]));
+    return RTXPT_OK;
+}
+extern "C" RTXPT_API int rtxpt_b200_last_env_update_ms(rtxpt_ctx* c, float* outMs4)
+{
+    if (!c || !outMs4) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    memcpy(outMs4, c->envUpdateMs, sizeof(c->envUpdateMs));
     return RTXPT_OK;
 }
 

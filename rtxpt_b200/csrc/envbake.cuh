@@ -120,4 +120,79 @@ PT_HD void mipReduceTexel(const Params& p, uint mip, uint x, uint y, uint face)
     storeTexel(texelAt(p, mip, face, x, y), weightedAverage(make_float4(a[0], a[1], a[2], a[3]), make_float4(b[0], b[1], b[2], b[3]), make_float4(c[0], c[1], c[2], c[3]), make_float4(d[0], d[1], d[2], d[3]), w));
 }
 
+// ---- importance / radiance map of a re-baked cube (BuildMIPDescentImportanceMapCS, EnvMapImportanceSamplingBaker.hlsl:56-90, + the 2x2 box MIP chain after it) ----------------
+// A second implementation of LightBaker::buildEnvRadianceMap (lights_bake.cpp), on purpose: the host one serves the scene upload, this one rtxpt_b200_update_env_map.  Every
+// operation follows the host's order (face selection, 8-bit bilinear weights, per-face clamp, summation order, fp16 rounding), so the host build of these bodies equals the host map
+// bit for bit (tests/test_env_update.py).  On the GPU the cos / sin of the octahedral mapping come from libdevice and the host's from the C library; neither is correctly
+// rounded, so the two maps differ in a small share of texels and the upload keeps the host map (the light tables of an upload stay those the oracle holds bit for bit).
+constexpr uint kImportanceDim = 1024, kImportanceMips = 11, kImportanceSamples = 4;       // EMISB_IMPORTANCE_MAP_DIM, EMISB_IMPORTANCE_SAMPLES_PER_PIXEL^2 = 16 taps
+struct ImportanceParams
+{
+    const float* cube; uint faceSize;                       // MIP 0 of the bake: 6 faces of faceSize^2 RGBA32F texels
+    float* mips[kImportanceMips];                           // MIP m: (1024 >> m)^2 RGBA32F texels holding fp16 values (.a = importance)
+};
+PT_HD float3 octEqualAreaToDirHD(float u, float v)      // oct_to_ndir_equal_area_unorm with the host's constant and sign function
+{
+    const float px = u * 2.f - 1.f, py = v * 2.f - 1.f;
+    const float d = 1.f - (fabsf(px) + fabsf(py));
+    const float r = 1.f - fabsf(d);
+    const float phi = (r > 0.f) ? ((fabsf(py) - fabsf(px)) / r + 1.f) * 0.78539816339744830961f : 0.f;
+    const float f = r * sqrtf(2.f - r * r);
+    const float sx = (px > 0.f) ? 1.f : ((px < 0.f) ? -1.f : 0.f), sy = (py > 0.f) ? 1.f : ((py < 0.f) ? -1.f : 0.f), sd = (d > 0.f) ? 1.f : ((d < 0.f) ? -1.f : 0.f);
+    return mk3(f * sx * cosf(phi), f * sy * sinf(phi), sd * (1.f - r * r));
+}
+PT_HD float q8(float a) { return floorf(a * 256.0f + 0.5f) * (1.0f / 256.0f); }        // 8 fractional bits, like the texture units
+PT_HD float3 cubeTexel(const ImportanceParams& p, uint face, int x, int y)
+{
+    const int n = int(p.faceSize);
+    x = clampi(x, 0, n - 1); y = clampi(y, 0, n - 1);
+    const float* t = p.cube + ((size_t(face) * n + y) * n + x) * 4;
+    return mk3(t[0], t[1], t[2]);
+}
+PT_HD float3 sampleCubeMip0(const ImportanceParams& p, float3 v)
+{
+    const float ax = fabsf(v.x), ay = fabsf(v.y), az = fabsf(v.z);
+    float m, s, t; uint face;
+    if (ax >= ay && ax >= az) { m = ax; if (v.x >= 0) { face = 0; s = -v.z; t = -v.y; } else { face = 1; s = v.z; t = -v.y; } }
+    else if (ay >= az)        { m = ay; if (v.y >= 0) { face = 2; s = v.x; t = v.z; }  else { face = 3; s = v.x; t = -v.z; } }
+    else                      { m = az; if (v.z >= 0) { face = 4; s = v.x; t = -v.y; } else { face = 5; s = -v.x; t = -v.y; } }
+    const float n = float(p.faceSize);
+    const float x = (s / m + 1.0f) * 0.5f * n - 0.5f, y = (t / m + 1.0f) * 0.5f * n - 0.5f;
+    const float fx = floorf(x), fy = floorf(y);
+    const float wx = q8(x - fx), wy = q8(y - fy);
+    const int ix = int(fx), iy = int(fy);
+    const float3 a = cubeTexel(p, face, ix, iy) * (1 - wx) + cubeTexel(p, face, ix + 1, iy) * wx;
+    const float3 b = cubeTexel(p, face, ix, iy + 1) * (1 - wx) + cubeTexel(p, face, ix + 1, iy + 1) * wx;
+    return a * (1 - wy) + b * wy;
+}
+// texel (px, py) of MIP 0: 4 x 4 taps, radiance and (luminance + average) / 2 importance
+PT_HD void importanceTexel(const ImportanceParams& p, uint px, uint py)
+{
+    const uint N = kImportanceDim, S = kImportanceSamples;
+    const float inv = 1.0f / float(S * S);
+    float L = 0.f; float3 R = mk3(0.f);
+    for (uint y = 0; y < S; y++)
+        for (uint x = 0; x < S; x++)
+        {
+            const float3 dir = octEqualAreaToDirHD((float(px * S + x) + 0.5f) / float(N * S), (float(py * S + y) + 0.5f) / float(N * S));
+            const float3 rad = sampleCubeMip0(p, dir);
+            const float lum = rad.x * 0.2126f + rad.y * 0.7152f + rad.z * 0.0722f, avg = (rad.x + rad.y + rad.z) / 3.0f;
+            L += (lum + avg) * 0.5f;
+            R = R + rad;
+        }
+    float* o = p.mips[0] + (size_t(py) * N + px) * 4;
+    o[0] = lpf(R.x * inv); o[1] = lpf(R.y * inv); o[2] = lpf(R.z * inv); o[3] = lpf(L * inv);
+}
+// texel (x, y) of MIP m >= 1: the 2x2 box of MIP m - 1 (donut's MipMapGenPass, MODE_COLOR)
+PT_HD void importanceReduceTexel(const ImportanceParams& p, uint mip, uint x, uint y)
+{
+    const uint n = kImportanceDim >> mip, pn = kImportanceDim >> (mip - 1);
+    const float* src = p.mips[mip - 1];
+    for (uint c = 0; c < 4; c++)
+    {
+        const float s = src[(size_t(2 * y) * pn + 2 * x) * 4 + c] + src[(size_t(2 * y) * pn + 2 * x + 1) * 4 + c] + src[(size_t(2 * y + 1) * pn + 2 * x) * 4 + c] + src[(size_t(2 * y + 1) * pn + 2 * x + 1) * 4 + c];
+        p.mips[mip][(size_t(y) * n + x) * 4 + c] = lpf(s * 0.25f);
+    }
+}
+
 } } // namespace pt::envbake

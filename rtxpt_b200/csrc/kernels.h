@@ -54,8 +54,9 @@ namespace tonemap { struct Params; }
 void launchToneMap(const tonemap::Params& p, const void* src, bool srcIsF32, uint32_t pixelCount, double* partials, float* avgLuminance, uint32_t* dst, cudaStream_t s);      // tonemap_kernels.cu
 namespace refit { struct Params; }
 void launchRefit(const refit::Params& p, const uint32_t* levelStart, uint32_t levelCount, int smCount, cudaStream_t s);      // refit_kernels.cu
-namespace envbake { struct Params; }
+namespace envbake { struct Params; struct ImportanceParams; }
 void launchEnvBake(const envbake::Params& p, uint32_t mipLevels, cudaStream_t s);                  // envbake_kernels.cu: EnvMapBaker BaseLayerCS + MIPReduceCS
+void launchEnvImportance(const envbake::ImportanceParams& p, cudaStream_t s);                      // envbake_kernels.cu: BuildMIPDescentImportanceMapCS + its 2x2 MIP chain
 namespace neeat { struct Params; }
 void launchNeeatUpdateBegin(const neeat::Params& p, bool preFilter, uint* scanBlockSums, int smCount, cudaStream_t s);     // neeat_kernels.cu
 void launchNeeatUpdateEnd(const neeat::Params& p, cudaStream_t s);

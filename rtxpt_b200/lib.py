@@ -61,6 +61,8 @@ _SIGNATURES = {
     "rtxpt_b200_rebuild_bvh": [C.c_void_p, C.c_void_p],
     "rtxpt_b200_get_bvh_stats": [C.c_void_p, C.POINTER(S.BvhStats)],
     "rtxpt_b200_bake_env_map": [C.c_void_p, C.POINTER(S.EnvBakeDesc), C.c_void_p, C.c_size_t],
+    "rtxpt_b200_update_env_map": [C.c_void_p, C.POINTER(S.EnvBakeDesc), C.c_void_p],
+    "rtxpt_b200_last_env_update_ms": [C.c_void_p, C.POINTER(C.c_float)],
     "rtxpt_b200_neeat_update_begin": [C.c_void_p, C.c_void_p],
     "rtxpt_b200_neeat_update_end": [C.c_void_p, C.c_void_p],
     "rtxpt_b200_get_opacity_mask_stats": [C.c_void_p, C.POINTER(S.OpacityMaskStats)],
@@ -253,11 +255,24 @@ def split_env_mips(flat, cube_dim):
     return out
 
 
-def _bake_env_map(call, cube_dim, source, source_type, scale_color, lights):
-    src, st, w, h, lt = env_bake_arguments(cube_dim, source, source_type, scale_color, lights)
+def split_importance_mips(flat, dim=1024):
+    """The radiance / importance MIP chain (scene_raw(8)) as a list of n x n x 4 arrays, 1024^2 down to 1^2."""
+    out = []; off = 0; n = dim
+    while n > 0:
+        cnt = n * n * 4; out.append(flat[off: off + cnt].reshape(n, n, 4)); off += cnt; n //= 2
+    return out
+
+
+def _env_bake_desc(cube_dim, src, st, w, h, lt, scale_color):
     d = S.EnvBakeDesc(); d.cubeDim = cube_dim; d.sourceType = st; d.sourceWidth = w; d.sourceHeight = h; d.source = None if src is None else src.ctypes.data
     d.scaleColor[:] = list(scale_color); d.directionalLightCount = len(lt)
     for i in range(len(lt)): d.lights[i].colorIntensity[:] = lt[i, :4].tolist(); d.lights[i].direction[:] = lt[i, 4:7].tolist(); d.lights[i].angularSize = float(lt[i, 7])
+    return d
+
+
+def _bake_env_map(call, cube_dim, source, source_type, scale_color, lights):
+    src, st, w, h, lt = env_bake_arguments(cube_dim, source, source_type, scale_color, lights)
+    d = _env_bake_desc(cube_dim, src, st, w, h, lt, scale_color)
     total = sum(6 * (cube_dim >> m) ** 2 * 4 for m in range(cube_dim.bit_length()))
     out = np.zeros(total, np.float32)
     call(d, out)
@@ -365,11 +380,12 @@ class Context:
         _check(self.L.rtxpt_b200_skin_update(self.h, skin_id, m.ctypes.data, len(m), stream), self.L)
 
     # (dtype, words per row) of rtxpt_b200_debug_scene_readback's buffers; 4 (the instance table) is returned as structs.InstanceData
-    _SCENE_RAW = {0: (np.uint32, 20), 1: (np.uint32, 12), 2: (np.uint32, 24), 3: (np.float32, 9), 5: (np.uint32, 1), 6: (np.float32, 6)}
+    _SCENE_RAW = {0: (np.uint32, 20), 1: (np.uint32, 12), 2: (np.uint32, 24), 3: (np.float32, 9), 5: (np.uint32, 1), 6: (np.float32, 6), 7: (np.float32, 1), 8: (np.float32, 1), 9: (np.uint32, 1)}
 
     def scene_raw(self, what):
-        """Tests / debugging: the scene state on the device (0 BVH nodes, 1 leaf triangles, 2 shade records, 3 previous positions, 4 instances, 5 level starts, 6 exact node boxes);
-        one row per node / triangle / record, level starts as a flat array."""
+        """Tests / debugging: the scene state on the device (0 BVH nodes, 1 leaf triangles, 2 shade records, 3 previous positions, 4 instances, 5 level starts, 6 exact node boxes,
+        7 environment cube MIPs, 8 radiance / importance MIPs, 9 environment lookup map); one row per node / triangle / record, flat arrays for 5, 7, 8 and 9
+        (split_env_mips / split_importance_mips cut 7 and 8 into MIPs)."""
         n = C.c_size_t()
         _check(self.L.rtxpt_b200_debug_scene_readback(self.h, what, None, 0, C.byref(n)), self.L)
         if what == 4:
@@ -411,6 +427,22 @@ class Context:
         """EnvMapBaker on the GPU.  source: HxWx4 float32 equirectangular image or 6xNxNx4 cube (None = lights only); lights: (colour rgb, intensity W/sr, incoming direction,
         angular size rad) tuples.  Returns the MIP chain as a list of 6 x n x n x 4 float32 arrays (what SceneBuilder.set_env_cube / RtxptEnvCubeDesc take)."""
         return _bake_env_map(lambda d, out: _check(self.L.rtxpt_b200_bake_env_map(self.h, C.byref(d), out.ctypes.data, out.size), self.L), cube_dim, source, source_type, scale_color, lights)
+
+    def update_env_map(self, cube_dim, source=None, source_type=None, scale_color=(1.0, 1.0, 1.0), lights=(), kept_source=None, stream=None):
+        """Re-bakes the environment of the uploaded scene on the GPU (rtxpt_b200_update_env_map): same arguments as bake_env_map.  kept_source=(source_type, width, height)
+        instead of `source` re-bakes from the source the context kept from its last update (an equirectangular W x H image: (1, W, H); a cube of N^2 faces: (2, N, N))."""
+        if kept_source is not None:
+            if source is not None: raise ValueError("give either source or kept_source")
+            (st, w, h), src, lt = kept_source, None, env_bake_arguments(cube_dim, None, None, scale_color, lights)[4]
+        else:
+            src, st, w, h, lt = env_bake_arguments(cube_dim, source, source_type, scale_color, lights)
+        d = _env_bake_desc(cube_dim, src, st, w, h, lt, scale_color)
+        _check(self.L.rtxpt_b200_update_env_map(self.h, C.byref(d), stream), self.L)
+
+    def last_env_update_ms(self):
+        """Event times of the last update_env_map (ms): dict of bake, importance, copy, host (read-back + host light bake + upload)."""
+        t = (C.c_float * 4)(); _check(self.L.rtxpt_b200_last_env_update_ms(self.h, t), self.L)
+        return dict(zip(("bake", "importance", "copy", "host"), [float(x) for x in t]))
 
     # ---- NEE-AT temporal feedback: per frame set_constants; neeat_update_begin; path_trace_realtime (runs update_end after its BUILD pass) ----
     def opacity_mask_stats(self):
