@@ -711,7 +711,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
     }
     // a pixel's feedback reservoir is updated by one path at a time, as in the reference's sequential sub-sample dispatches: no batching while feedback is active
     const uint32_t subSamplesPerLaunch = na ? 1u : c->cfg.maxSubSamplesPerLaunch;
-    queryOccupancy(c->grid, 16 + size_t(p.smemNodeCount) * 80);
+    const TraceKind shadowKind = na ? TraceKind::ShadowNeeat : TraceKind::Shadow;
     const bool countSteps = (c->cfg.flags & RTXPT_CFG_COUNT_TRAVERSAL_STEPS) != 0;
     const bool hasRefraction = c->consts.nestedDielectricsQuality > 0;
     const uint32_t iterations = std::min<uint32_t>(c->consts.bounceCount + 1 + (hasRefraction ? 4 : 0), kMaxWavefrontIterations);
@@ -759,17 +759,17 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
             {
                 q.iteration = it;
                 if (it > 0) std::swap(q.stateIn, q.stateOut);     // the paths k_shade(it - 1) appended are iteration it's rays
-                ktl.begin(0); launchTraceClosest(q, c->grid, countSteps, ls); ktl.end();
+                ktl.begin(0); launchTrace(TraceKind::Closest, q, c->grid, countSteps, ls); ktl.end();
                 if (overlap && it > 0) CU(cudaStreamWaitEvent(ls, L.evShadowDone, 0));        // shadow(it-1) has updated the radiance words
                 ktl.begin(2); if (na) launchShadeNeeat(q, c->grid, ls); else launchShade(q, c->grid, ls); ktl.end();
                 if (overlap)
                 {
                     CU(cudaEventRecord(L.evShadeDone, ls));
                     CU(cudaStreamWaitEvent(ls2, L.evShadeDone, 0));
-                    if (na) launchTraceShadowNeeat(q, c->grid, ls2); else launchTraceShadow(q, c->grid, countSteps, ls2);
+                    launchTrace(shadowKind, q, c->grid, countSteps, ls2);
                     CU(cudaEventRecord(L.evShadowDone, ls2));
                 }
-                else { ktl.begin(1); if (na) launchTraceShadowNeeat(q, c->grid, ls); else launchTraceShadow(q, c->grid, countSteps, ls); ktl.end(); }
+                else { ktl.begin(1); launchTrace(shadowKind, q, c->grid, countSteps, ls); ktl.end(); }
                 launches += 3;
             }
             if (overlap) CU(cudaStreamWaitEvent(ls, L.evShadowDone, 0));
@@ -857,7 +857,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
     for (uint32_t it = 0; it < buildIterations; it++)
     {
         p.iteration = it;
-        launchTraceClosestRealtime(p, c->grid, s); launchRtShade(p, c->grid, false, s); launches += 2;
+        launchTrace(TraceKind::ClosestRealtime, p, c->grid, false, s); launchRtShade(p, c->grid, false, s); launches += 2;
     }
     if (na)
     {   // LightsBaker::UpdateEnd sits between the BUILD pass (this frame's depth and motion vectors) and the radiance passes (Sample.cpp:2495)
@@ -876,9 +876,9 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
         for (uint32_t it = 0; it < fillIterations; it++)
         {
             p.iteration = it;
-            launchTraceClosestRealtime(p, c->grid, s);
-            if (na) { launchRtShadeNeeat(p, c->grid, s); launchTraceShadowRealtimeNeeat(p, c->grid, s); }
-            else { launchRtShade(p, c->grid, true, s); launchTraceShadowRealtime(p, c->grid, s); }
+            launchTrace(TraceKind::ClosestRealtime, p, c->grid, false, s);
+            if (na) { launchRtShadeNeeat(p, c->grid, s); launchTrace(TraceKind::ShadowRealtimeNeeat, p, c->grid, false, s); }
+            else { launchRtShade(p, c->grid, true, s); launchTrace(TraceKind::ShadowRealtime, p, c->grid, false, s); }
             launches += 3;
         }
         launchRtFillCommit(p, c->grid, s); launches++;
@@ -1754,7 +1754,6 @@ extern "C" RTXPT_API int rtxpt_b200_trace_rays_device(rtxpt_ctx* c, const void* 
     cudaSetDevice(c->device);
     if (c->counters.count == 0) CU(c->counters.alloc(size_t(kCounterWords) * rtxpt_ctx::kMaxLanes));
     LaunchParams p; fillParams(c, p);
-    queryOccupancy(c->grid, 16 + size_t(p.smemNodeCount) * 80);
     CU(cudaMemsetAsync(c->counters.ptr, 0, 8, c->stream));
     if (repeat == 0) repeat = 1;
     CU(cudaEventRecord(c->evStart, c->stream));

@@ -74,11 +74,7 @@ __global__ void __launch_bounds__(256) k_generate(const __grid_constant__ Launch
     }
 }
 
-// ---- closest hit ------------------------------------------------------------------------------------------------------------------------
-// Persistent warps with dynamic ray fetch: a lane whose ray has finished writes its hit, bins the path into its shade queue and pulls the
-// next ray from the queue cursor; lanes still traversing resume where they stopped.  Keeps SIMT lanes busy although ray lengths differ
-// by an order of magnitude.
-
+// ---- traversal loop -----------------------------------------------------------------------------------------------------------------------
 // shared memory of the traversal kernels: [mbarrier 16 B][WarpScratch x 8 warps][staged BVH nodes]
 #ifndef PT_TRACE_THREADS
 #define PT_TRACE_THREADS 256     // threads per traversal CTA; the resident-CTA count scales so that warps per SM stay the same
@@ -87,48 +83,37 @@ constexpr uint kTraceThreads = PT_TRACE_THREADS, kTraceCtaScale = 256 / PT_TRACE
 constexpr uint kTraceWarps = kTraceThreads / 32;
 constexpr uint kTraceScratchBytes = 16 + kTraceWarps * sizeof(WarpScratch);
 
-// RAY_ORDER (reference mode): ray i is entry i of p.stateIn and writes hits[i]; otherwise (realtime) the ray queue names the path slot
-template <bool COUNT, int MINB, bool RAY_ORDER>
-__global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_closest(const __grid_constant__ LaunchParams p)
+// Persistent warps with dynamic ray fetch, shared by every traversal kernel: a lane whose ray has finished retires it and pulls the next
+// ray index from `fetchCursor` (one atomic per warp); lanes still traversing resume where they stopped.  Keeps SIMT lanes busy although
+// ray lengths differ by an order of magnitude.  Rays 0 .. count-1 are traced; the callers differ only in the two inlined callbacks:
+//   fetchRay(i, o, d, tMin, tMax)  loads ray i and keeps what the caller needs when the ray retires
+//   retireRay(retireMask, ws)      called by every lane whose ray has finished, with its result in ws (Traverser::result); with RETIRE_MASK
+//                                  retireMask is the ballot of those lanes, for warp-collective work among them (0 otherwise: no vote is taken)
+// Returns this thread's traversal counters (zero unless COUNT).
+template <bool ANY_HIT, bool COUNT, bool RETIRE_MASK, typename FetchRay, typename RetireRay>
+PT_DEVICE TraversalCounters traceLoop(const LaunchParams& p, uint* fetchCursor, uint count, FetchRay&& fetchRay, RetireRay&& retireRay)
 {
     extern __shared__ __align__(16) unsigned char smemRaw[];
-    uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
-    const uint count = ctr[kCtrRayCount];
-    if (count == 0) return;                 // wavefront already drained (uniform across the grid)
     uint64_t* mbar = reinterpret_cast<uint64_t*>(smemRaw);
     WarpScratch& ws = reinterpret_cast<WarpScratch*>(smemRaw + 16)[threadIdx.x >> 5];
     uint4* smemNodes = reinterpret_cast<uint4*>(smemRaw + kTraceScratchBytes);
     stageNodesToShared(smemNodes, p.scene.bvhNodes, p.smemNodeCount, mbar);
 
-    const uint* __restrict__ queue = p.wf.rayQueue[p.iteration & 1];
     TraversalCounters tc; tc.nodeVisits = 0; tc.triTests = 0;
     const uint lane = threadIdx.x & 31u, laneLt = (1u << lane) - 1u;
-    Traverser<false, COUNT> tv; tv.done = true; tv.waiting = false;
+    Traverser<ANY_HIT, COUNT> tv; tv.done = true; tv.waiting = false;
     uint2 stack[kTraversalStackSize];
     uint head = 0, tail = 0;
     if (lane == 0) ws.tail = 0;
     __syncwarp();
-    bool hasRay = false, exhausted = false; uint entry = 0;
+    bool hasRay = false, exhausted = false;
     while (true)
     {
-        // retire finished rays: hit record + SER-style binning by {miss, terminating hit, material class}
         const bool retire = tv.done && hasRay;
-        const uint retireMask = __ballot_sync(0xFFFFFFFFu, retire);
+        const uint retireMask = RETIRE_MASK ? __ballot_sync(0xFFFFFFFFu, retire) : 0u;
         if (retire)
         {
-            const uint slot = entry & 0x7FFFFFFFu;
-            uint subInstance; const HitRecord h = tv.result(ws, subInstance);
-            p.wf.hits[slot] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
-            uint cls;
-            if (h.gid == 0xFFFFFFFFu) cls = 0;
-            else if (entry & 0x80000000u) cls = 1;
-            else cls = (p.flags & RTXPT_CFG_NO_MATERIAL_SORT) ? 2u : 2u + p.scene.subInstanceClass[subInstance];
-            const uint peers = __match_any_sync(retireMask, cls);
-            const uint leader = __ffs(peers) - 1u;
-            uint base = 0;
-            if (lane == leader) base = atomicAdd(ctr + kCtrShadeCount + cls, __popc(peers));
-            base = __shfl_sync(peers, base, leader);
-            p.wf.shadeQueue[size_t(cls) * p.wf.capacity + base + __popc(peers & laneLt)] = slot;
+            retireRay(retireMask, ws);
             hasRay = false;
         }
         // fetch the next ray for every idle lane with one atomic per warp
@@ -138,7 +123,7 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
         {
             const uint leader = __ffs(fetchMask) - 1u;
             uint base = 0;
-            if (lane == leader) base = atomicAdd(ctr + kCtrFetchClosest, __popc(fetchMask));
+            if (lane == leader) base = atomicAdd(fetchCursor, __popc(fetchMask));
             base = __shfl_sync(0xFFFFFFFFu, base, leader);
             if (fetch)
             {
@@ -146,19 +131,9 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
                 if (i >= count) exhausted = true;
                 else
                 {
-                    uint4 a, b;
-                    if constexpr (RAY_ORDER)
-                    {   // the sign bit of s1.w is the path's kPFTerminateAtNextBounce (wavefront.cuh)
-                        a = ldState(p.stateIn.s0 + i); b = ldState(p.stateIn.s1 + i);
-                        entry = i | (b.w & 0x80000000u);
-                    }
-                    else
-                    {
-                        entry = queue[i];
-                        const uint slot = entry & 0x7FFFFFFFu;
-                        a = ldState(p.wf.s0 + slot); b = ldState(p.wf.s1 + slot);
-                    }
-                    tv.init(p.scene, ws, mk3(__uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z)), mk3(__uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z)), 0.0f, kMaxRayTravel);
+                    float3 o, d; float tMin, tMax;
+                    fetchRay(i, o, d, tMin, tMax);
+                    tv.init(p.scene, ws, o, d, tMin, tMax);
                     hasRay = true;
                 }
             }
@@ -168,6 +143,55 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
         const bool drained = __any_sync(0xFFFFFFFFu, exhausted);
         tv.run(p.scene, p.scene.bvhNodes, smemNodes, p.smemNodeCount, drained ? 1 : p.refillThreshold, p.waitFlushLanes, &tc, stack, ws, head, tail);
     }
+    return tc;
+}
+
+// ---- closest hit ------------------------------------------------------------------------------------------------------------------------
+// A retiring lane writes its hit and bins the path into its shade queue.
+// RAY_ORDER (reference mode): ray i is entry i of p.stateIn and writes hits[i]; otherwise (realtime) the ray queue names the path slot
+template <bool COUNT, int MINB, bool RAY_ORDER>
+__global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_closest(const __grid_constant__ LaunchParams p)
+{
+    uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
+    const uint count = ctr[kCtrRayCount];
+    if (count == 0) return;                 // wavefront already drained (uniform across the grid)
+    const uint* __restrict__ queue = p.wf.rayQueue[p.iteration & 1];
+    uint entry = 0;
+    auto fetchRay = [&](uint i, float3& o, float3& d, float& tMin, float& tMax)
+    {
+        uint4 a, b;
+        if constexpr (RAY_ORDER)
+        {   // the sign bit of s1.w is the path's kPFTerminateAtNextBounce (wavefront.cuh)
+            a = ldState(p.stateIn.s0 + i); b = ldState(p.stateIn.s1 + i);
+            entry = i | (b.w & 0x80000000u);
+        }
+        else
+        {
+            entry = queue[i];
+            const uint slot = entry & 0x7FFFFFFFu;
+            a = ldState(p.wf.s0 + slot); b = ldState(p.wf.s1 + slot);
+        }
+        o = mk3(__uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z)); d = mk3(__uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z));
+        tMin = 0.0f; tMax = kMaxRayTravel;
+    };
+    auto retireRay = [&](uint retireMask, const WarpScratch& ws)
+    {   // hit record + SER-style binning by {miss, terminating hit, material class}
+        const uint lane = threadIdx.x & 31u, laneLt = (1u << lane) - 1u;
+        const uint slot = entry & 0x7FFFFFFFu;
+        uint subInstance; const HitRecord h = Traverser<false, COUNT>::result(ws, subInstance);
+        p.wf.hits[slot] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
+        uint cls;
+        if (h.gid == 0xFFFFFFFFu) cls = 0;
+        else if (entry & 0x80000000u) cls = 1;
+        else cls = (p.flags & RTXPT_CFG_NO_MATERIAL_SORT) ? 2u : 2u + p.scene.subInstanceClass[subInstance];
+        const uint peers = __match_any_sync(retireMask, cls);
+        const uint leader = __ffs(peers) - 1u;
+        uint base = 0;
+        if (lane == leader) base = atomicAdd(ctr + kCtrShadeCount + cls, __popc(peers));
+        base = __shfl_sync(peers, base, leader);
+        p.wf.shadeQueue[size_t(cls) * p.wf.capacity + base + __popc(peers & laneLt)] = slot;
+    };
+    const TraversalCounters tc = traceLoop<false, COUNT, true>(p, ctr + kCtrFetchClosest, count, fetchRay, retireRay);
     if (COUNT) { atomicAdd(ctr + kCtrNodeVisits, tc.nodeVisits); atomicAdd(ctr + kCtrTriTests, tc.triTests); }
 }
 
@@ -177,95 +201,58 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
 template <bool COUNT, int MINB, bool REALTIME = false, bool NEEAT = false>
 __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_shadow(const __grid_constant__ LaunchParams p)
 {
-    extern __shared__ __align__(16) unsigned char smemRaw[];
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
     const uint frontCount = ctr[kCtrShadowCount], count = frontCount + ctr[kCtrShadowShort];      // long rays first (wavefront.cuh: appendShadowRecord)
     if (count == 0) return;
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(smemRaw);
-    WarpScratch& ws = reinterpret_cast<WarpScratch*>(smemRaw + 16)[threadIdx.x >> 5];
-    uint4* smemNodes = reinterpret_cast<uint4*>(smemRaw + kTraceScratchBytes);
-    stageNodesToShared(smemNodes, p.scene.bvhNodes, p.smemNodeCount, mbar);
-
-    TraversalCounters tc; tc.nodeVisits = 0; tc.triTests = 0;
-    uint visibleCount = 0;
-    const uint lane = threadIdx.x & 31u, laneLt = (1u << lane) - 1u;
-    Traverser<true, COUNT> tv; tv.done = true; tv.waiting = false;
-    uint2 stack[kTraversalStackSize];
-    uint head = 0, tail = 0;
-    if (lane == 0) ws.tail = 0;
-    __syncwarp();
-    bool hasRay = false, exhausted = false; uint record = 0, slot = 0;
-    while (true)
+    uint visibleCount = 0, record = 0, slot = 0;
+    auto fetchRay = [&](uint i, float3& o, float3& d, float& tMin, float& tMax)
     {
-        if (tv.done && hasRay)
+        record = shadowRecordIndex(i, frontCount, p.wf.capacity);
+        const float4 ot = p.wf.shadowOriginTMax[record], dp = p.wf.shadowDirPath[record];
+        slot = __float_as_uint(dp.w);
+        o = mk3(ot.x, ot.y, ot.z); d = mk3(dp.x, dp.y, dp.z); tMin = 0.0f; tMax = ot.w;
+    };
+    auto retireRay = [&](uint, const WarpScratch& ws)
+    {
+        if (uint(ws.bestKey[threadIdx.x & 31u]) != 0xFFFFFFFFu) return;
+        // visible: HandleHit's "if any(neeRadianceAndSpecAvg > 0) AccumulatePathRadiance" (PathTracer.hlsli:725-746)
+        const uint2 r = p.wf.shadowRadiance[record];
+        const float rx = f16tof32(r.x & 0x7FFFu), ry = f16tof32((r.x >> 16) & 0x7FFFu), rz = f16tof32(r.y), rw = f16tof32(r.y >> 16);
+        if (rx > 0 || ry > 0 || rz > 0 || rw > 0)
         {
-            if (uint(ws.bestKey[lane]) == 0xFFFFFFFFu)
-            {   // visible: HandleHit's "if any(neeRadianceAndSpecAvg > 0) AccumulatePathRadiance" (PathTracer.hlsli:725-746)
-                const uint2 r = p.wf.shadowRadiance[record];
-                const float rx = f16tof32(r.x & 0x7FFFu), ry = f16tof32((r.x >> 16) & 0x7FFFu), rz = f16tof32(r.y), rw = f16tof32(r.y >> 16);
-                if (rx > 0 || ry > 0 || rz > 0 || rw > 0)
-                {
-                    if constexpr (REALTIME)
-                    {
-                        uint4 s2 = p.wf.s2[slot];
-                        const float a = p.rt.attenuation;
-                        const float spec = (r.x & 0x00008000u) ? rw : ((r.x & 0x80000000u) ? (rx + ry + rz) / 3.0f : 0.0f);
-                        const float lx = f16tof32(s2.z) + rx * a, ly = f16tof32(s2.z >> 16) + ry * a, lz = f16tof32(s2.w) + rz * a, lw = f16tof32(s2.w >> 16) + spec * a;
-                        s2.z = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
-                        s2.w = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
-                        p.wf.s2[slot] = s2;
-                    }
-                    else
-                    {   // reference mode: `slot` is the path's home index h
-                        uint2 l = p.radiance[slot];
-                        const float lx = f16tof32(l.x) + rx, ly = f16tof32(l.x >> 16) + ry, lz = f16tof32(l.y) + rz, lw = f16tof32(l.y >> 16);
-                        l.x = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
-                        l.y = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
-                        p.radiance[slot] = l;
-                    }
-                }
-                if constexpr (NEEAT)
-                {   // the light was visible: the pixel's feedback reservoir hears about it (PathTracerNEE.hlsli:276-283) and the path's next shade takes the roulette
-                    // outcome that belongs to a visible sample (shade.cuh)
-                    const uint4 fb = p.naShadowFeedback[record];
-                    if (fb.w & 0x80000000u)
-                    {
-                        const uint id = p.wf.pixelOfSlot[slot];
-                        neeat::Reservoir::at(p.na.fbWeight, p.na.fbCandidate, size_t(id & 0xFFFFu) * p.na.W + (id >> 16)).add(__uint_as_float(fb.z), fb.x & 0x7FFFFFFFu, __uint_as_float(fb.y), (fb.x & 0x80000000u) != 0);
-                        p.naRrFix[slot] = fb.w;
-                    }
-                }
-                visibleCount++;
-            }
-            hasRay = false;
-        }
-        const bool fetch = tv.done && !exhausted;
-        const uint fetchMask = __ballot_sync(0xFFFFFFFFu, fetch);
-        if (fetchMask)
-        {
-            const uint leader = __ffs(fetchMask) - 1u;
-            uint base = 0;
-            if (lane == leader) base = atomicAdd(ctr + kCtrFetchShadow, __popc(fetchMask));
-            base = __shfl_sync(0xFFFFFFFFu, base, leader);
-            if (fetch)
+            if constexpr (REALTIME)
             {
-                record = base + __popc(fetchMask & laneLt);
-                if (record >= count) exhausted = true;
-                else
-                {
-                    record = shadowRecordIndex(record, frontCount, p.wf.capacity);
-                    const float4 ot = p.wf.shadowOriginTMax[record], dp = p.wf.shadowDirPath[record];
-                    slot = __float_as_uint(dp.w);
-                    tv.init(p.scene, ws, mk3(ot.x, ot.y, ot.z), mk3(dp.x, dp.y, dp.z), 0.0f, ot.w);
-                    hasRay = true;
-                }
+                uint4 s2 = p.wf.s2[slot];
+                const float a = p.rt.attenuation;
+                const float spec = (r.x & 0x00008000u) ? rw : ((r.x & 0x80000000u) ? (rx + ry + rz) / 3.0f : 0.0f);
+                const float lx = f16tof32(s2.z) + rx * a, ly = f16tof32(s2.z >> 16) + ry * a, lz = f16tof32(s2.w) + rz * a, lw = f16tof32(s2.w >> 16) + spec * a;
+                s2.z = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
+                s2.w = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
+                p.wf.s2[slot] = s2;
+            }
+            else
+            {   // reference mode: `slot` is the path's home index h
+                uint2 l = p.radiance[slot];
+                const float lx = f16tof32(l.x) + rx, ly = f16tof32(l.x >> 16) + ry, lz = f16tof32(l.y) + rz, lw = f16tof32(l.y >> 16);
+                l.x = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
+                l.y = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
+                p.radiance[slot] = l;
             }
         }
-        __syncwarp();
-        if (__all_sync(0xFFFFFFFFu, tv.done && !hasRay)) break;
-        const bool drained = __any_sync(0xFFFFFFFFu, exhausted);
-        tv.run(p.scene, p.scene.bvhNodes, smemNodes, p.smemNodeCount, drained ? 1 : p.refillThreshold, p.waitFlushLanes, &tc, stack, ws, head, tail);
-    }
+        if constexpr (NEEAT)
+        {   // the light was visible: the pixel's feedback reservoir hears about it (PathTracerNEE.hlsli:276-283) and the path's next shade takes the roulette
+            // outcome that belongs to a visible sample (shade.cuh)
+            const uint4 fb = p.naShadowFeedback[record];
+            if (fb.w & 0x80000000u)
+            {
+                const uint id = p.wf.pixelOfSlot[slot];
+                neeat::Reservoir::at(p.na.fbWeight, p.na.fbCandidate, size_t(id & 0xFFFFu) * p.na.W + (id >> 16)).add(__uint_as_float(fb.z), fb.x & 0x7FFFFFFFu, __uint_as_float(fb.y), (fb.x & 0x80000000u) != 0);
+                p.naRrFix[slot] = fb.w;
+            }
+        }
+        visibleCount++;
+    };
+    const TraversalCounters tc = traceLoop<true, COUNT, false>(p, ctr + kCtrFetchShadow, count, fetchRay, retireRay);
     if (COUNT) { atomicAdd(ctr + kCtrShadowNodeVisits, tc.nodeVisits); atomicAdd(ctr + kCtrShadowTriTests, tc.triTests); atomicAdd(ctr + kCtrShadowVisible, visibleCount); }
 }
 
@@ -298,59 +285,26 @@ __global__ void __launch_bounds__(256) k_commit_accumulate(const __grid_constant
     }
 }
 
-// ---- standalone ray queries (parity tests, traversal benchmark): same Traverser and dynamic fetch as the wavefront kernels ------------------
+// ---- standalone ray queries (parity tests, traversal benchmark): the wavefront kernels' traversal loop -------------------------------------
 template <bool ANY_HIT>
 __global__ void __launch_bounds__(kTraceThreads, 2 * kTraceCtaScale) k_trace_rays(const __grid_constant__ LaunchParams p, const RtxptRay* __restrict__ rays, uint count, RtxptHit* __restrict__ out, uint* counters, uint* cursor)
 {
-    extern __shared__ __align__(16) unsigned char smemRaw[];
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(smemRaw);
-    WarpScratch& ws = reinterpret_cast<WarpScratch*>(smemRaw + 16)[threadIdx.x >> 5];
-    uint4* smemNodes = reinterpret_cast<uint4*>(smemRaw + kTraceScratchBytes);
-    stageNodesToShared(smemNodes, p.scene.bvhNodes, p.smemNodeCount, mbar);
-    TraversalCounters tc; tc.nodeVisits = 0; tc.triTests = 0;
-    const uint lane = threadIdx.x & 31u, laneLt = (1u << lane) - 1u;
-    Traverser<ANY_HIT, true> tv; tv.done = true; tv.waiting = false;
-    uint2 stack[kTraversalStackSize];
-    uint head = 0, tail = 0;
-    if (lane == 0) ws.tail = 0;
-    __syncwarp();
-    bool hasRay = false, exhausted = false; uint index = 0;
-    while (true)
+    uint index = 0;
+    auto fetchRay = [&](uint i, float3& o, float3& d, float& tMin, float& tMax)
     {
-        if (tv.done && hasRay)
-        {
-            uint subInstance; const HitRecord h = tv.result(ws, subInstance);
-            RtxptHit r;
-            if (h.gid != 0xFFFFFFFFu) { const uint4 info = p.scene.triInfo[h.gid]; r.t = h.t; r.u = h.u; r.v = h.v; r.instanceIndex = info.x; r.geometryIndex = info.y; r.primitiveIndex = info.z; }
-            else { r.t = -1.0f; r.u = r.v = 0.f; r.instanceIndex = r.geometryIndex = r.primitiveIndex = 0xFFFFFFFFu; }
-            out[index] = r;
-            hasRay = false;
-        }
-        const bool fetch = tv.done && !exhausted;
-        const uint fetchMask = __ballot_sync(0xFFFFFFFFu, fetch);
-        if (fetchMask)
-        {
-            const uint leader = __ffs(fetchMask) - 1u;
-            uint base = 0;
-            if (lane == leader) base = atomicAdd(cursor, __popc(fetchMask));
-            base = __shfl_sync(0xFFFFFFFFu, base, leader);
-            if (fetch)
-            {
-                index = base + __popc(fetchMask & laneLt);
-                if (index >= count) exhausted = true;
-                else
-                {
-                    const float4 a = reinterpret_cast<const float4*>(rays)[index * 2], b = reinterpret_cast<const float4*>(rays)[index * 2 + 1];
-                    tv.init(p.scene, ws, mk3(a.x, a.y, a.z), mk3(b.x, b.y, b.z), a.w, b.w);
-                    hasRay = true;
-                }
-            }
-        }
-        __syncwarp();
-        if (__all_sync(0xFFFFFFFFu, tv.done && !hasRay)) break;
-        const bool drained = __any_sync(0xFFFFFFFFu, exhausted);
-        tv.run(p.scene, p.scene.bvhNodes, smemNodes, p.smemNodeCount, drained ? 1 : p.refillThreshold, p.waitFlushLanes, &tc, stack, ws, head, tail);
-    }
+        index = i;
+        const float4 a = reinterpret_cast<const float4*>(rays)[i * 2], b = reinterpret_cast<const float4*>(rays)[i * 2 + 1];
+        o = mk3(a.x, a.y, a.z); d = mk3(b.x, b.y, b.z); tMin = a.w; tMax = b.w;
+    };
+    auto retireRay = [&](uint, const WarpScratch& ws)
+    {
+        uint subInstance; const HitRecord h = Traverser<ANY_HIT, true>::result(ws, subInstance);
+        RtxptHit r;
+        if (h.gid != 0xFFFFFFFFu) { const uint4 info = p.scene.triInfo[h.gid]; r.t = h.t; r.u = h.u; r.v = h.v; r.instanceIndex = info.x; r.geometryIndex = info.y; r.primitiveIndex = info.z; }
+        else { r.t = -1.0f; r.u = r.v = 0.f; r.instanceIndex = r.geometryIndex = r.primitiveIndex = 0xFFFFFFFFu; }
+        out[index] = r;
+    };
+    const TraversalCounters tc = traceLoop<ANY_HIT, true, false>(p, cursor, count, fetchRay, retireRay);
     if (counters) { atomicAdd(counters + 0, tc.nodeVisits); atomicAdd(counters + 1, tc.triTests); }
 }
 
@@ -429,27 +383,42 @@ void launchUnpackAll(const float4* srcAll, const uint32_t* allPixelTable, uint32
 // ---- launch wrappers ---------------------------------------------------------------------------------------------------------------------------
 static size_t traceSmemBytes(const LaunchParams& p) { return kTraceScratchBytes + size_t(p.smemNodeCount) * 80; }
 
+// Every wavefront traversal instantiation, one row per TraceKind.  Column 0 counts traversal steps (MINB 2, reference mode only); columns 1..3 are
+// MINB 2..4, the resident CTAs per SM the kernel's registers are capped for.  nullptr: no such instantiation.
+using TraceKernel = void (*)(LaunchParams);
+static const TraceKernel kTraceKernels[][4] = {
+    { k_trace_closest<true, 2, true>, k_trace_closest<false, 2, true>,       k_trace_closest<false, 3, true>,  k_trace_closest<false, 4, true> },        // Closest
+    { nullptr,                        k_trace_closest<false, 2, false>,      k_trace_closest<false, 3, false>, k_trace_closest<false, 4, false> },       // ClosestRealtime
+    { k_trace_shadow<true, 2>,        k_trace_shadow<false, 2>,              k_trace_shadow<false, 3>,         k_trace_shadow<false, 4> },               // Shadow
+    { nullptr,                        k_trace_shadow<false, 2, true>,        nullptr,                          k_trace_shadow<false, 4, true> },         // ShadowRealtime
+    { nullptr,                        k_trace_shadow<false, 2, false, true>, nullptr,                          k_trace_shadow<false, 4, false, true> },  // ShadowNeeat
+    { nullptr,                        k_trace_shadow<false, 2, true, true>,  nullptr,                          k_trace_shadow<false, 4, true, true> },   // ShadowRealtimeNeeat
+};
+static_assert(sizeof(kTraceKernels) / sizeof(kTraceKernels[0]) == size_t(TraceKind::Count), "one table row per TraceKind");
+
 template <typename K> static cudaError_t allowSmem(K kernel, int bytes) { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); }
 
 cudaError_t configureKernels(int maxSmemOptin)
 {
     cudaError_t e;
     const int want = maxSmemOptin > 0 ? maxSmemOptin : 0;
-#define ALLOW(k) if ((e = allowSmem(k, want)) != cudaSuccess) return e
-    ALLOW((k_trace_closest<false, 2, true>)); ALLOW((k_trace_closest<false, 3, true>)); ALLOW((k_trace_closest<false, 4, true>)); ALLOW((k_trace_closest<true, 2, true>));
-    ALLOW((k_trace_closest<false, 2, false>)); ALLOW((k_trace_closest<false, 3, false>)); ALLOW((k_trace_closest<false, 4, false>));
-    ALLOW((k_trace_shadow<false, 2>)); ALLOW((k_trace_shadow<false, 3>)); ALLOW((k_trace_shadow<false, 4>)); ALLOW((k_trace_shadow<true, 2>));
-    ALLOW((k_trace_shadow<false, 4, true>)); ALLOW((k_trace_shadow<false, 2, true>));
-    ALLOW((k_trace_shadow<false, 4, true, true>)); ALLOW((k_trace_shadow<false, 2, true, true>)); ALLOW((k_trace_shadow<false, 4, false, true>)); ALLOW((k_trace_shadow<false, 2, false, true>));
-    ALLOW(k_trace_rays<false>); ALLOW(k_trace_rays<true>);
-#undef ALLOW
-    return cudaSuccess;
+    for (const auto& row : kTraceKernels)
+        for (TraceKernel k : row)
+            if (k && (e = allowSmem(k, want)) != cudaSuccess) return e;
+    if ((e = allowSmem(k_trace_rays<false>, want)) != cudaSuccess) return e;
+    return allowSmem(k_trace_rays<true>, want);
 }
 
-// launch with the optional L2 access-policy window of GridConfig attached as a per-launch attribute (no stream state is touched)
-template <typename K> static void launchTrace(K kernel, int grid, size_t smem, cudaStream_t s, const LaunchParams& p, const GridConfig& g)
+// launched with the optional L2 access-policy window of GridConfig attached as a per-launch attribute (no stream state is touched)
+void launchTrace(TraceKind kind, const LaunchParams& p, const GridConfig& g, bool countSteps, cudaStream_t s)
 {
-    cudaLaunchConfig_t cfg = {}; cfg.gridDim = dim3(uint(grid) * kTraceCtaScale); cfg.blockDim = dim3(kTraceThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    const TraceKernel* row = kTraceKernels[int(kind)];
+    const int minb = std::min(std::max(g.traceBlocksPerSM, 2), 4);
+    TraceKernel kernel = row[minb - 1];
+    int grid = g.smCount * g.traceBlocksPerSM;
+    if (countSteps && row[0]) kernel = row[0];
+    else if (!row[2] && minb < 4) { kernel = row[1]; grid = g.smCount * 2; }       // no MINB-3 instantiation: below four CTAs per SM, MINB 2 on two per SM
+    cudaLaunchConfig_t cfg = {}; cfg.gridDim = dim3(uint(grid) * kTraceCtaScale); cfg.blockDim = dim3(kTraceThreads); cfg.dynamicSmemBytes = traceSmemBytes(p); cfg.stream = s;
     cudaLaunchAttribute attr[1]; cfg.attrs = attr; cfg.numAttrs = 0;
     if (g.l2WindowBytes)
     {
@@ -463,57 +432,12 @@ template <typename K> static void launchTrace(K kernel, int grid, size_t smem, c
 }
 
 void launchGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_generate<<<g.smCount * 4, 256, 0, s>>>(p); }
-void launchTraceClosest(const LaunchParams& p, const GridConfig& g, bool count, cudaStream_t s)
-{
-    const int grid = g.smCount * g.traceBlocksPerSM; const size_t smem = traceSmemBytes(p);
-    if (count) launchTrace(k_trace_closest<true, 2, true>, grid, smem, s, p, g);
-    else if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_closest<false, 4, true>, grid, smem, s, p, g);
-    else if (g.traceBlocksPerSM == 3) launchTrace(k_trace_closest<false, 3, true>, grid, smem, s, p, g);
-    else launchTrace(k_trace_closest<false, 2, true>, grid, smem, s, p, g);
-}
-void launchTraceClosestRealtime(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
-{
-    const int grid = g.smCount * g.traceBlocksPerSM; const size_t smem = traceSmemBytes(p);
-    if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_closest<false, 4, false>, grid, smem, s, p, g);
-    else if (g.traceBlocksPerSM == 3) launchTrace(k_trace_closest<false, 3, false>, grid, smem, s, p, g);
-    else launchTrace(k_trace_closest<false, 2, false>, grid, smem, s, p, g);
-}
-void launchTraceShadow(const LaunchParams& p, const GridConfig& g, bool count, cudaStream_t s)
-{
-    const int grid = g.smCount * g.traceBlocksPerSM; const size_t smem = traceSmemBytes(p);
-    if (count) launchTrace(k_trace_shadow<true, 2>, grid, smem, s, p, g);
-    else if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_shadow<false, 4>, grid, smem, s, p, g);
-    else if (g.traceBlocksPerSM == 3) launchTrace(k_trace_shadow<false, 3>, grid, smem, s, p, g);
-    else launchTrace(k_trace_shadow<false, 2>, grid, smem, s, p, g);
-}
-void launchTraceShadowRealtime(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
-{
-    const int grid = g.smCount * g.traceBlocksPerSM; const size_t smem = traceSmemBytes(p);
-    if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_shadow<false, 4, true>, grid, smem, s, p, g);
-    else launchTrace(k_trace_shadow<false, 2, true>, g.smCount * 2, smem, s, p, g);
-}
-void launchTraceShadowNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
-{
-    const int grid = g.smCount * g.traceBlocksPerSM; const size_t smem = traceSmemBytes(p);
-    if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_shadow<false, 4, false, true>, grid, smem, s, p, g);
-    else launchTrace(k_trace_shadow<false, 2, false, true>, g.smCount * 2, smem, s, p, g);
-}
-void launchTraceShadowRealtimeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
-{
-    const int grid = g.smCount * g.traceBlocksPerSM; const size_t smem = traceSmemBytes(p);
-    if (g.traceBlocksPerSM >= 4) launchTrace(k_trace_shadow<false, 4, true, true>, grid, smem, s, p, g);
-    else launchTrace(k_trace_shadow<false, 2, true, true>, g.smCount * 2, smem, s, p, g);
-}
 void launchCommitAccumulate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_commit_accumulate<<<g.smCount * 4, 256, 0, s>>>(p); }
 void launchTraceRays(const LaunchParams& p, const GridConfig& g, const RtxptRay* rays, uint32_t count, bool anyHit, RtxptHit* out, uint32_t* counters, uint32_t* cursor, cudaStream_t s)
 {
     cudaMemsetAsync(cursor, 0, sizeof(uint32_t), s);
     if (anyHit) k_trace_rays<true><<<g.smCount * g.traceBlocksPerSM * kTraceCtaScale, kTraceThreads, traceSmemBytes(p), s>>>(p, rays, count, out, counters, cursor);
     else k_trace_rays<false><<<g.smCount * g.traceBlocksPerSM * kTraceCtaScale, kTraceThreads, traceSmemBytes(p), s>>>(p, rays, count, out, counters, cursor);
-}
-void queryOccupancy(GridConfig& g, size_t smemBytes)
-{
-    (void)g; (void)smemBytes;    // traceBlocksPerSM is chosen by the caller together with the shared-memory node budget
 }
 
 } // namespace pt

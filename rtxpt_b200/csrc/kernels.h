@@ -13,17 +13,16 @@ struct GridConfig
 };
 
 cudaError_t configureKernels(int maxSmemOptin);
-void queryOccupancy(GridConfig& g, size_t traceSmemBytes);
 void launchGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
-void launchTraceClosest(const LaunchParams& p, const GridConfig& g, bool countSteps, cudaStream_t s);           // reference mode: rays in state order
+// wavefront traversal (kernels.cu): closest-hit or shadow rays; reference mode takes rays in state order, realtime mode through the slot queue;
+// the NEE-AT shadow kinds also feed visible samples back to the pixel's reservoir.  countSteps selects the step-counting kernel of Closest and Shadow.
+enum class TraceKind { Closest, ClosestRealtime, Shadow, ShadowRealtime, ShadowNeeat, ShadowRealtimeNeeat, Count };
+void launchTrace(TraceKind kind, const LaunchParams& p, const GridConfig& g, bool countSteps, cudaStream_t s);
 void launchShade(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
-void launchTraceShadow(const LaunchParams& p, const GridConfig& g, bool countSteps, cudaStream_t s);
-// realtime mode (realtime_kernels.cu; the shadow kernel variant lives with the other traversal kernels)
+// realtime mode (realtime_kernels.cu)
 void launchRtBuildGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtFillGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtShade(const LaunchParams& p, const GridConfig& g, bool fill, cudaStream_t s);
-void launchTraceClosestRealtime(const LaunchParams& p, const GridConfig& g, cudaStream_t s);                    // realtime mode: rays through the slot queue
-void launchTraceShadowRealtime(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtFillCommit(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchDnPrepareInputs(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
@@ -38,9 +37,7 @@ void launchDebugRng(const uint32_t* dIn, uint32_t count, uint32_t* dOut, cudaStr
 
 void launchDnSpecHitT(const float* src, const float* depth, float* dst, int W, int H, cudaStream_t s);      // DenoisingGuidesBaker::DenoiseSpecHitT, one pass
 void launchShadeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s);                 // reference-mode shade with NEE-AT feedback (shade_kernels.cu)
-void launchTraceShadowNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtShadeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s);               // FILL pass shade with NEE-AT feedback (realtime_kernels.cu)
-void launchTraceShadowRealtimeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s);   // + feedback insertion for visible samples (kernels.cu)
 namespace skin { struct Params; }
 constexpr uint32_t kExchangeMaxImages = 8;
 struct ExchangeSet { void* image[kExchangeMaxImages]; uint32_t bytesPerPixel[kExchangeMaxImages]; uint64_t segmentOffset[kExchangeMaxImages]; uint64_t bytesPerRank; uint32_t count, width; };
