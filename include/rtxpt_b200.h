@@ -235,7 +235,11 @@ typedef struct RtxptPathTracerConstants {
     uint32_t NEEEnabled;
     uint32_t NEEType;                       /* 0 uniform, 1 power, 2 NEE-AT (see NEEATFeedback) */
     uint32_t NEECandidateSamples;
-    uint32_t NEEFullSamples;
+    uint32_t NEEFullSamples;                /* light samples per path vertex, each with its own shadow ray (SampleUI "Full samples", 1 by default); values above 63 act as 63, 0
+                                             * takes none.  N > 1: a path_trace launch batches max(1, maxSubSamplesPerLaunch / N) sub-samples, and the first trace allocates
+                                             * about 56 B x N per path of such a launch (RTXPT_ERR_OUT_OF_MEMORY if that fails; the context keeps working with N = 1).
+                                             * N > 1 with NEEType 2 and NEEATFeedback is refused (RTXPT_ERR_UNSUPPORTED): a visible sample's feedback draw would decide the
+                                             * next sample's candidates. */
     uint32_t enableRussianRoulette;         /* PT_ENABLE_RUSSIAN_ROULETTE macro, Sample.cpp:988-1042 */
     uint32_t enableLDSamplerForBSDF;        /* RTXPT_ENABLE_LOW_DISCREPANCY_SAMPLER_FOR_BSDF */
     uint32_t nestedDielectricsQuality;      /* RTXPT_NESTED_DIELECTRICS_QUALITY: 0 off, 1 fast */
@@ -531,7 +535,7 @@ RTXPT_API uint32_t rtxpt_b200_generic_ts_address(uint32_t x, uint32_t y, uint32_
 
 typedef struct RtxptStats {
     uint64_t scatterRays;           /* closest-hit queries of the last path_trace call */
-    uint64_t shadowRays;            /* any-hit (visibility) queries */
+    uint64_t shadowRays;            /* any-hit (visibility) queries: one per valid light sample */
     uint64_t paths;
     uint64_t kernelLaunches;        /* kernels launched by the last path_trace call */
     uint64_t traversalNodeVisits;   /* closest-hit queries; only with RTXPT_CFG_COUNT_TRAVERSAL_STEPS */
@@ -540,7 +544,7 @@ typedef struct RtxptStats {
     uint64_t shadowTriTests;
     uint64_t raysPerBounce[16];     /* scatter rays per wavefront iteration */
     float    msTotal;               /* CUDA-event time of the last path_trace call */
-    float    msTraceClosest, msTraceShadow, msShade, msOther;
+    float    msTraceClosest, msTraceShadow, msShade, msOther;     /* msOther: camera rays, commit and, with NEEFullSamples > 1, the NEE resolve */
     uint32_t bvhNodeCount, bvhTriangleCount;
     float    bvhBuildSeconds;
     uint32_t lightCount, lightProxyCount;

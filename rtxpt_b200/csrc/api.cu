@@ -139,6 +139,8 @@ struct rtxpt_ctx
     DeviceArray<uint4> s0, s1, s2, s3, s4; DeviceArray<float4> hits; DeviceArray<uint32_t> rayQueue[2], shadeQueue;
     DeviceArray<uint4> t0, t1, t2, t3, t4; DeviceArray<uint2> radiance;        // reference mode: second path-state set, radiance per home index (wavefront.cuh)
     DeviceArray<float4> shadowOriginTMax, shadowDirPath; DeviceArray<uint2> shadowRadiance;
+    // NEEFullSamples > 1: shadow records of every light sample and the NEE blocks (wavefront.cuh), allocated by the first trace that needs them (ensureNeeSamples)
+    struct NeeSamples { DeviceArray<float4> originTMax, dirPath; DeviceArray<uint2> sample; DeviceArray<uint4> blocks; } neeSamples;
     DeviceArray<uint32_t> counters; DeviceArray<uint32_t> pixelOfSlot, allPixelTable;
     uint32_t paddedPixelsPerRank = 0;
     uint32_t capacity = 0, pixelCount = 0, tableWidth = 0, tableHeight = 0;
@@ -620,7 +622,9 @@ extern "C" RTXPT_API int rtxpt_b200_set_constants(rtxpt_ctx* c, const RtxptPathT
 {
     if (!c || !k) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
     cudaSetDevice(c->device);
-    if (k->NEEFullSamples > 1) return fail(RTXPT_ERR_UNSUPPORTED, "NEEFullSamples > 1 is not supported in this tier (one shadow record per vertex)");
+    if (k->NEEFullSamples > 1 && k->NEEType == 2 && k->NEEATFeedback != 0)
+        return fail(RTXPT_ERR_UNSUPPORTED, "NEEFullSamples > 1 together with NEE-AT temporal feedback is not supported: a visible sample's feedback draw decides the next sample's candidates, "
+                                           "and the wavefront learns visibility only after the shadow kernel");
     if (k->bounceCount + 6 > (uint32_t)kMaxWavefrontIterations) return fail(RTXPT_ERR_UNSUPPORTED, "bounceCount above %d", kMaxWavefrontIterations - 6);
     int rc = ensureTargets(c, k->imageWidth, k->imageHeight);
     if (rc != RTXPT_OK) return rc;
@@ -693,6 +697,36 @@ static int checkReady(rtxpt_ctx* c)
     return RTXPT_OK;
 }
 
+// NEEFullSamples = N > 1: every vertex may emit N shadow records and owns an NEE block of 1 + N uint4, so a launch batches max(1, maxSubSamplesPerLaunch / N)
+// sub-samples (include/rtxpt_b200.h) and the multi-sample arrays hold that many paths' records and blocks
+static uint32_t neeFullSamples(const rtxpt_ctx* c) { return std::min(kNeeMaxFullSamples, c->consts.NEEFullSamples); }
+static uint32_t multiSampleSubSamples(const rtxpt_ctx* c) { const uint32_t n = neeFullSamples(c); return n > 1 ? std::max(1u, c->cfg.maxSubSamplesPerLaunch / n) : c->cfg.maxSubSamplesPerLaunch; }
+static int ensureNeeSamples(rtxpt_ctx* c)
+{
+    const uint32_t n = neeFullSamples(c);
+    const size_t paths = size_t(multiSampleSubSamples(c)) * c->pixelCount, records = paths * n, blocks = paths * (1 + n);
+    if (records >= 0x7FFFFFFFull || blocks >= 0xFFFFFFFFull) return fail(RTXPT_ERR_UNSUPPORTED, "NEEFullSamples %u: too many shadow records per launch", n);
+    rtxpt_ctx::NeeSamples& a = c->neeSamples;
+    if (a.originTMax.count >= records && a.blocks.count >= blocks) return RTXPT_OK;
+    CU(syncContext(c));                 // earlier launches may still read the arrays being replaced
+    cudaError_t e;
+    if ((e = a.originTMax.alloc(records)) != cudaSuccess || (e = a.dirPath.alloc(records)) != cudaSuccess || (e = a.sample.alloc(records)) != cudaSuccess || (e = a.blocks.alloc(blocks)) != cudaSuccess)
+    {   // nothing half-allocated stays behind, and the failed allocation is not reported again by a later launch: the context keeps rendering with fewer samples
+        a = rtxpt_ctx::NeeSamples();
+        cudaGetLastError();
+        return fail(e == cudaErrorMemoryAllocation ? RTXPT_ERR_OUT_OF_MEMORY : RTXPT_ERR_CUDA, "NEEFullSamples %u: %zu shadow records and %zu NEE block words: %s", n, records, blocks, cudaGetErrorString(e));
+    }
+    return RTXPT_OK;
+}
+// point a launch's shadow records and NEE blocks at the multi-sample arrays, from path `first` on; the launch's p.wf.capacity paths own N records each (neeShadowCapacity)
+static void useNeeSamples(rtxpt_ctx* c, LaunchParams& p, size_t first)
+{
+    const uint32_t n = neeFullSamples(c);
+    WavefrontBuffers& w = p.wf;
+    w.shadowOriginTMax = c->neeSamples.originTMax.ptr + first * n; w.shadowDirPath = c->neeSamples.dirPath.ptr + first * n; w.shadowRadiance = c->neeSamples.sample.ptr + first * n;
+    p.neeBlocks = c->neeSamples.blocks.ptr + first * (1 + n);
+}
+
 static bool neeatActive(const rtxpt_ctx* c);
 extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSampleIndex, uint32_t subSampleCount, int accumulate, void* cudaStream)
 {
@@ -709,9 +743,11 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
         p.na = c->na.params; p.naShadowFeedback = c->na.shadowFeedback.ptr; p.naRrFix = c->na.rrFix.ptr;
         p.scene.proxyCounters = c->na.proxyCounters.ptr; p.scene.proxyIndices = c->na.proxyIndices.ptr;
     }
+    const bool multi = neeFullSamples(c) > 1;          // (never together with feedback: rtxpt_b200_set_constants)
+    if (multi) { rc = ensureNeeSamples(c); if (rc != RTXPT_OK) return rc; }
     // a pixel's feedback reservoir is updated by one path at a time, as in the reference's sequential sub-sample dispatches: no batching while feedback is active
-    const uint32_t subSamplesPerLaunch = na ? 1u : c->cfg.maxSubSamplesPerLaunch;
-    const TraceKind shadowKind = na ? TraceKind::ShadowNeeat : TraceKind::Shadow;
+    const uint32_t subSamplesPerLaunch = na ? 1u : multiSampleSubSamples(c);
+    const TraceKind shadowKind = na ? TraceKind::ShadowNeeat : (multi ? TraceKind::ShadowMulti : TraceKind::Shadow);
     const bool countSteps = (c->cfg.flags & RTXPT_CFG_COUNT_TRAVERSAL_STEPS) != 0;
     const bool hasRefraction = c->consts.nestedDielectricsQuality > 0;
     const uint32_t iterations = std::min<uint32_t>(c->consts.bounceCount + 1 + (hasRefraction ? 4 : 0), kMaxWavefrontIterations);
@@ -744,6 +780,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
                 if (na) { q.naShadowFeedback += o; q.naRrFix += o; }
                 for (StateSet* st : { &q.stateIn, &q.stateOut }) { st->s0 += o; st->s1 += o; st->s2 += o; st->s3 += o; st->s4 += o; }
                 q.radiance += o;
+                if (multi) useNeeSamples(c, q, o);
             }
             q.firstSampleIndex = c->consts.sampleBaseIndex + firstSubSampleIndex + done + firstSub;
             q.subSampleCount = count;
@@ -767,10 +804,15 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
                     CU(cudaEventRecord(L.evShadeDone, ls));
                     CU(cudaStreamWaitEvent(ls2, L.evShadeDone, 0));
                     launchTrace(shadowKind, q, c->grid, countSteps, ls2);
+                    if (multi) launchNeeResolve(q, c->grid, false, ls2);          // the visible samples' radiance, before k_shade(it+1) reads it
                     CU(cudaEventRecord(L.evShadowDone, ls2));
                 }
-                else { ktl.begin(1); launchTrace(shadowKind, q, c->grid, countSteps, ls); ktl.end(); }
-                launches += 3;
+                else
+                {
+                    ktl.begin(1); launchTrace(shadowKind, q, c->grid, countSteps, ls); ktl.end();
+                    if (multi) { ktl.begin(3); launchNeeResolve(q, c->grid, false, ls); ktl.end(); }
+                }
+                launches += multi ? 4 : 3;
             }
             if (overlap) CU(cudaStreamWaitEvent(ls, L.evShadowDone, 0));
             if (l > 0) CU(cudaStreamWaitEvent(ls, c->lanes[l - 1].evCommitted, 0));       // the running mean takes the sub-samples in order
@@ -839,6 +881,8 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
     cudaStream_t s = pickStream(c, cudaStream);
     const bool na = neeatActive(c);
     if (na && (!c->na.allocated || !c->na.frameBegun)) return fail(RTXPT_ERR_INVALID_ARGUMENT, "NEEATFeedback is set: call rtxpt_b200_neeat_update_begin before tracing the frame");
+    const bool multi = neeFullSamples(c) > 1;
+    if (multi) { rc = ensureNeeSamples(c); if (rc != RTXPT_OK) return rc; }
     LaunchParams p; fillParams(c, p);
     const RtxptRealtimeConstants& r = c->realtime;
     fillRealtimeParams(c, p);
@@ -866,6 +910,11 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
         p.scene.proxyCounters = c->na.proxyCounters.ptr; p.scene.proxyIndices = c->na.proxyIndices.ptr;
         launches += 4;
     }
+    if (multi)
+    {   // the FILL pass traces one path per pixel: the shade queues and the light samples' records are laid out for that many paths
+        p.wf.capacity = std::max(c->pixelCount, 1u);
+        useNeeSamples(c, p, 0);
+    }
     for (uint32_t sub = 0; sub < r.subSampleCount; sub++)
     {
         p.firstSampleIndex = c->consts.sampleBaseIndex + sub;
@@ -878,6 +927,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
             p.iteration = it;
             launchTrace(TraceKind::ClosestRealtime, p, c->grid, false, s);
             if (na) { launchRtShadeNeeat(p, c->grid, s); launchTrace(TraceKind::ShadowRealtimeNeeat, p, c->grid, false, s); }
+            else if (multi) { launchRtShade(p, c->grid, true, s); launchTrace(TraceKind::ShadowRealtimeMulti, p, c->grid, false, s); launchNeeResolve(p, c->grid, true, s); launches++; }
             else { launchRtShade(p, c->grid, true, s); launchTrace(TraceKind::ShadowRealtime, p, c->grid, false, s); }
             launches += 3;
         }

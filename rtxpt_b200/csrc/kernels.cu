@@ -198,7 +198,8 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
 // ---- shadow rays ----------------------------------------------------------------------------------------------------------------------------
 // REALTIME (FILL pass of realtime mode): the radiance is attenuated by 1 / sub-sample count and comes with a specular average chosen by the shade
 // kernel (sign bits of the record's first word, shade.cuh) - AccumulatePathRadiance of PATH_TRACER_MODE_FILL_STABLE_PLANES (PathTracer.hlsli:145-159)
-template <bool COUNT, int MINB, bool REALTIME = false, bool NEEAT = false>
+// MULTI (NEEFullSamples > 1): a record is one light sample of a vertex; a visible one sets its bit in the vertex's NEE block and leaves L to k_nee_resolve
+template <bool COUNT, int MINB, bool REALTIME = false, bool NEEAT = false, bool MULTI = false>
 __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_shadow(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
@@ -207,7 +208,7 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
     uint visibleCount = 0, record = 0, slot = 0;
     auto fetchRay = [&](uint i, float3& o, float3& d, float& tMin, float& tMax)
     {
-        record = shadowRecordIndex(i, frontCount, p.wf.capacity);
+        record = shadowRecordIndex(i, frontCount, MULTI ? neeShadowCapacity(p) : p.wf.capacity);
         const float4 ot = p.wf.shadowOriginTMax[record], dp = p.wf.shadowDirPath[record];
         slot = __float_as_uint(dp.w);
         o = mk3(ot.x, ot.y, ot.z); d = mk3(dp.x, dp.y, dp.z); tMin = 0.0f; tMax = ot.w;
@@ -217,28 +218,8 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
         if (uint(ws.bestKey[threadIdx.x & 31u]) != 0xFFFFFFFFu) return;
         // visible: HandleHit's "if any(neeRadianceAndSpecAvg > 0) AccumulatePathRadiance" (PathTracer.hlsli:725-746)
         const uint2 r = p.wf.shadowRadiance[record];
-        const float rx = f16tof32(r.x & 0x7FFFu), ry = f16tof32((r.x >> 16) & 0x7FFFu), rz = f16tof32(r.y), rw = f16tof32(r.y >> 16);
-        if (rx > 0 || ry > 0 || rz > 0 || rw > 0)
-        {
-            if constexpr (REALTIME)
-            {
-                uint4 s2 = p.wf.s2[slot];
-                const float a = p.rt.attenuation;
-                const float spec = (r.x & 0x00008000u) ? rw : ((r.x & 0x80000000u) ? (rx + ry + rz) / 3.0f : 0.0f);
-                const float lx = f16tof32(s2.z) + rx * a, ly = f16tof32(s2.z >> 16) + ry * a, lz = f16tof32(s2.w) + rz * a, lw = f16tof32(s2.w >> 16) + spec * a;
-                s2.z = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
-                s2.w = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
-                p.wf.s2[slot] = s2;
-            }
-            else
-            {   // reference mode: `slot` is the path's home index h
-                uint2 l = p.radiance[slot];
-                const float lx = f16tof32(l.x) + rx, ly = f16tof32(l.x >> 16) + ry, lz = f16tof32(l.y) + rz, lw = f16tof32(l.y >> 16);
-                l.x = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
-                l.y = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
-                p.radiance[slot] = l;
-            }
-        }
+        if constexpr (MULTI) atomicOr(reinterpret_cast<unsigned long long*>(&p.neeBlocks[slot].z), 1ull << r.x);     // `slot`: the block's header, r.x: the sample's index in the block
+        else accumulateNeeRadiance<REALTIME>(p, slot, r);
         if constexpr (NEEAT)
         {   // the light was visible: the pixel's feedback reservoir hears about it (PathTracerNEE.hlsli:276-283) and the path's next shade takes the roulette
             // outcome that belongs to a visible sample (shade.cuh)
@@ -254,6 +235,16 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
     };
     const TraversalCounters tc = traceLoop<true, COUNT, false>(p, ctr + kCtrFetchShadow, count, fetchRay, retireRay);
     if (COUNT) { atomicAdd(ctr + kCtrShadowNodeVisits, tc.nodeVisits); atomicAdd(ctr + kCtrShadowTriTests, tc.triTests); atomicAdd(ctr + kCtrShadowVisible, visibleCount); }
+}
+
+// ---- NEE resolve (NEEFullSamples > 1) --------------------------------------------------------------------------------------------------------------
+// after k_trace_shadow of the same iteration: one thread per NEE block sums the visible samples in sample order and applies the sum to the path (wavefront.cuh)
+template <bool REALTIME>
+__global__ void __launch_bounds__(256) k_nee_resolve(const __grid_constant__ LaunchParams p)
+{
+    const uint count = p.wf.counters[p.iteration * kCountersPerIter + kCtrNeeBlocks];
+    const uint stride = 1u + min(kNeeMaxFullSamples, p.c.NEEFullSamples);
+    for (uint b = blockIdx.x * blockDim.x + threadIdx.x; b < count; b += gridDim.x * blockDim.x) resolveNeeBlock<REALTIME>(p, p.neeBlocks + size_t(b) * stride);
 }
 
 // ---- commit + accumulate ---------------------------------------------------------------------------------------------------------------------
@@ -393,6 +384,8 @@ static const TraceKernel kTraceKernels[][4] = {
     { nullptr,                        k_trace_shadow<false, 2, true>,        nullptr,                          k_trace_shadow<false, 4, true> },         // ShadowRealtime
     { nullptr,                        k_trace_shadow<false, 2, false, true>, nullptr,                          k_trace_shadow<false, 4, false, true> },  // ShadowNeeat
     { nullptr,                        k_trace_shadow<false, 2, true, true>,  nullptr,                          k_trace_shadow<false, 4, true, true> },   // ShadowRealtimeNeeat
+    { nullptr, k_trace_shadow<false, 2, false, false, true>, nullptr, k_trace_shadow<false, 4, false, false, true> },                                         // ShadowMulti
+    { nullptr, k_trace_shadow<false, 2, true, false, true>,  nullptr, k_trace_shadow<false, 4, true, false, true> },                                          // ShadowRealtimeMulti
 };
 static_assert(sizeof(kTraceKernels) / sizeof(kTraceKernels[0]) == size_t(TraceKind::Count), "one table row per TraceKind");
 
@@ -433,6 +426,10 @@ void launchTrace(TraceKind kind, const LaunchParams& p, const GridConfig& g, boo
 
 void launchGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_generate<<<g.smCount * 4, 256, 0, s>>>(p); }
 void launchCommitAccumulate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_commit_accumulate<<<g.smCount * 4, 256, 0, s>>>(p); }
+void launchNeeResolve(const LaunchParams& p, const GridConfig& g, bool realtime, cudaStream_t s)
+{
+    if (realtime) k_nee_resolve<true><<<g.smCount * 4, 256, 0, s>>>(p); else k_nee_resolve<false><<<g.smCount * 4, 256, 0, s>>>(p);
+}
 void launchTraceRays(const LaunchParams& p, const GridConfig& g, const RtxptRay* rays, uint32_t count, bool anyHit, RtxptHit* out, uint32_t* counters, uint32_t* cursor, cudaStream_t s)
 {
     cudaMemsetAsync(cursor, 0, sizeof(uint32_t), s);

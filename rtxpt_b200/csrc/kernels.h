@@ -15,9 +15,11 @@ struct GridConfig
 cudaError_t configureKernels(int maxSmemOptin);
 void launchGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 // wavefront traversal (kernels.cu): closest-hit or shadow rays; reference mode takes rays in state order, realtime mode through the slot queue;
-// the NEE-AT shadow kinds also feed visible samples back to the pixel's reservoir.  countSteps selects the step-counting kernel of Closest and Shadow.
-enum class TraceKind { Closest, ClosestRealtime, Shadow, ShadowRealtime, ShadowNeeat, ShadowRealtimeNeeat, Count };
+// the NEE-AT shadow kinds also feed visible samples back to the pixel's reservoir; the Multi kinds (NEEFullSamples > 1) only mark visible samples in their NEE blocks,
+// which launchNeeResolve then applies.  countSteps selects the step-counting kernel of Closest and Shadow.
+enum class TraceKind { Closest, ClosestRealtime, Shadow, ShadowRealtime, ShadowNeeat, ShadowRealtimeNeeat, ShadowMulti, ShadowRealtimeMulti, Count };
 void launchTrace(TraceKind kind, const LaunchParams& p, const GridConfig& g, bool countSteps, cudaStream_t s);
+void launchNeeResolve(const LaunchParams& p, const GridConfig& g, bool realtime, cudaStream_t s);
 void launchShade(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 // realtime mode (realtime_kernels.cu)
 void launchRtBuildGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);

@@ -122,8 +122,10 @@ __global__ void __launch_bounds__(256) k_rt_fill_generate(const __grid_constant_
 #define PT_RT_SHADE_CTAS 4      // resident CTAs of 128 threads per SM: 4 caps the shade kernels at 128 registers (a few dozen bytes of spills), 3 lets them run without spills.
                                 // H100 SXM (700 W): config-3 trace 41.5 ms/frame with 4, 42.4 with 3; the 1-spp realtime frame 9.69 ms with 4, 9.60 with 3
 #endif
-template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false>
-__global__ void __launch_bounds__(128, PT_RT_SHADE_CTAS) k_rt_shade(const __grid_constant__ LaunchParams p)
+// MULTI (FILL pass, NEEFullSamples > 1): shadeHit appends the vertex's shadow records and NEE block itself, one record per valid light sample; 3 CTAs per SM, which
+// lets it run without spills in both builds
+template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false>
+__global__ void __launch_bounds__(128, MULTI ? 3 : PT_RT_SHADE_CTAS) k_rt_shade(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
     uint* ctrNext = ctr + kCountersPerIter;
@@ -145,7 +147,7 @@ __global__ void __launch_bounds__(128, PT_RT_SHADE_CTAS) k_rt_shade(const __grid
                 PathRegs path; path.load(p.wf, slot, true);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
                 if (cls == 0) shadeMiss<false, MODE, NEEAT>(p, path);
-                else shadeHit<false, ANALYTIC_LIGHTS, MODE, NEEAT>(p, path, slot, p.wf.hits[slot], out);
+                else shadeHit<false, ANALYTIC_LIGHTS, MODE, NEEAT, MULTI>(p, path, slot, p.wf.hits[slot], out);
                 continues = (cls != 0) && out.continuePath;
                 if constexpr (MODE == kModeBuildStablePlanes)
                 {   // postProcessHit: when this branch has ended, continue with the next enqueued branch of the pixel (planes above the current one)
@@ -161,7 +163,7 @@ __global__ void __launch_bounds__(128, PT_RT_SHADE_CTAS) k_rt_shade(const __grid
                 shadow = out.emitShadow;
             }
             appendRay(nextQueue, ctrNext + kCtrRayCount, continues, rayEntry);
-            if constexpr (MODE == kModeFillStablePlanes)
+            if constexpr (MODE == kModeFillStablePlanes && !MULTI)
             {
                 const uint b = appendShadowRecord(p, ctr, shadow, out.shadow.originTMax.w);
                 if (shadow)
@@ -266,6 +268,7 @@ void launchRtShade(const LaunchParams& p, const GridConfig& g, bool fill, cudaSt
 {
     const int grid = g.smCount * PT_RT_SHADE_CTAS;
     if (!fill) { if (p.scene.analyticLightCount != 0) k_rt_shade<kModeBuildStablePlanes, true><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeBuildStablePlanes, false><<<grid, 128, 0, s>>>(p); }
+    else if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1) k_rt_shade<kModeFillStablePlanes, true, false, true><<<g.smCount * 3, 128, 0, s>>>(p);      // several light samples per vertex: analytic lights gated at run time
     else { if (p.scene.analyticLightCount != 0) k_rt_shade<kModeFillStablePlanes, true><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeFillStablePlanes, false><<<grid, 128, 0, s>>>(p); }
 }
 void launchRtFillCommit(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_fill_commit<<<g.smCount * 4, 256, 0, s>>>(p); }

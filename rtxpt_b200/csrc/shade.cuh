@@ -10,7 +10,9 @@
 //                   (Lighting/LightSampler.hlsli:109-117, :282-328), TriangleLight / EnvironmentQuadLight
 //                   (Lighting/PolymorphicLight.hlsli:395-520, :560-640)
 // The NEE visibility ray is not traced here: the shade kernel emits a shadow record carrying the radiance "if visible" and the
-// shadow kernel adds it to L — same arithmetic and order as ProcessLightSample followed by AccumulatePathRadiance.
+// shadow kernel adds it to L — same arithmetic and order as ProcessLightSample followed by AccumulatePathRadiance.  With NEEFullSamples > 1
+// (MULTI) every valid light sample gets its own shadow record and parks its fp32 result in the vertex's NEE block (wavefront.cuh); the shadow
+// kernel marks the visible ones and k_nee_resolve sums them in sample order before the one AccumulatePathRadiance.
 #pragma once
 #include "wavefront.cuh"
 #include "bsdf.cuh"
@@ -490,7 +492,21 @@ PT_DEVICE void shadeMiss(const LaunchParams& p, PathRegs& path)
 // ---- hit -----------------------------------------------------------------------------------------------------------------------------------
 struct HitOutputs { bool continuePath; bool emitShadow; ShadowRecord shadow; uint4 naRecord; };     // naRecord: NEE-AT feedback of the shadow record (kernels with NEEAT = true)
 
-template <bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, int MODE = kModeReference, bool NEEAT = false>
+// FILL pass: which specular average AccumulatePathRadiance adds with the NEE radiance (PathTracer.hlsli:731-743), as the sign bits of the first word of the packed
+// (radiance, specAvg) - whose halves are non-negative: 00 none (the base scatter was diffuse), 01 the NEE result's own, 10 the average of the radiance.  ORed into `word`.
+PT_DEVICE void addFillSpecAvgChoice(uint& word, uint preFlags, uint preCounters)
+{
+    if (!(preFlags & (kPFStablePlaneBaseScatterDiff << kVertexIndexBits)))
+    {
+        const uint bouncesFromStablePlane = ((preCounters >> (kCtrBouncesFromStablePlane << 3)) & 0xffu) + 1u;
+        const bool special = (bouncesFromStablePlane == 1) || ((preFlags & (kPFDeltaOnlyPath << kVertexIndexBits)) && bouncesFromStablePlane <= 3);
+        word |= special ? 0x00008000u : 0x80000000u;
+    }
+}
+
+// MULTI: NEEFullSamples > 1 - the light samples' shadow records and the vertex's NEE block go straight to the launch's arrays (out.emitShadow stays false).  Without
+// NEE-AT feedback no draw depends on visibility, so the samples are drawn one after the other from the vertex's one uniform stream as HandleNEE draws them.
+template <bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, int MODE = kModeReference, bool NEEAT = false, bool MULTI = false>
 PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4 hit, HitOutputs& out)
 {
     out.continuePath = false; out.emitShadow = false;
@@ -689,17 +705,15 @@ PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4
         }
     }
 
-    // HandleNEE (PathTracerNEE.hlsli:303-346): candidates by weighted reservoir sampling, one shadow ray
+    // HandleNEE (PathTracerNEE.hlsli:303-346): per light sample, candidates by weighted reservoir sampling and one shadow ray
     uint neeMis = 0;
-    const uint fullSamples = min(63u, p.c.NEEFullSamples);      // this tier emits one shadow record per vertex: NEEFullSamples == 1 (reference default)
+    const uint fullSamples = min(kNeeMaxFullSamples, p.c.NEEFullSamples);      // kernels without MULTI run with NEEFullSamples <= 1 (the reference default): one shadow record per vertex
     uint naFeedback = 0xFFFFFFFFu; float naFeedbackWeight = 0.0f;          // NEEAT: the picked light (| ssc << 31) and how much the pixel wanted it
     if (p.c.NEEEnabled && (bsdfLobes(s.bsdf) & kLobeNonDelta) != 0 && (NEEAT ? *p.na.samplingProxyCount : p.scene.samplingProxyCount) != 0 && fullSamples > 0)
     {
         const uint candidateCount = p.c.NEECandidateSamples;
         const bool isSSC = (preConeWidth / preSceneLength) < (NEEAT ? p.na.screenSpaceVsWorldSpaceThreshold : 0.3f);
         neeMis = (1u << 15) | ((isSSC ? 1u : 0u) << 13) | ((candidateCount & 0x3F) << 6) | (fullSamples & 0x3F);
-        float3 pickLi = mk3(0.f), pickDir = mk3(0.f); float pickDist = 0.f, pickSelPdf = 0.f, pickSolidPdf = 0.f;
-        float weightSum = 0.f, pickWeight = 0.f; bool pickBsdfSampleable = true;
         const uint M = NEEAT ? *p.na.samplingProxyCount : p.scene.samplingProxyCount;
         const uint* __restrict__ proxyIndices = NEEAT ? p.na.proxyIndices : p.scene.proxyIndices;
         const uint* __restrict__ proxyCounters = NEEAT ? p.na.proxyCounters : p.scene.proxyCounters;
@@ -707,132 +721,148 @@ PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4
         // a frame of feedback has built the samplers)
         const uint localCount = (NEEAT && isSSC) ? neeat::candidateLocalCount(p.na.localToGlobalSampleRatio, candidateCount) : 0u, globalCount = candidateCount - localCount;
         const uint tileAddress = NEEAT ? neeat::localSamplingTilePos(p.na, path.id >> 16, path.id & 0xFFFFu) : 0u;
-        uint pickLight = 0xFFFFFFFFu; bool pickLocal = false;
-        // The candidate loop is a chain of dependent random gathers (proxy table -> counter, light record).  The light selection draws are
-        // every 4th value of the stream, so the proxy lookups of the first 8 candidates are issued up front and their light records
-        // prefetched into L2/L1 before the loop consumes them one by one.
-        constexpr uint kPrefetch = 8;
-        uint preLight[kPrefetch];
-        {
-            UniformSeq pre = uniformSG;
-            #pragma unroll
-            for (uint i = 0; i < kPrefetch; i++)
-            {
-                preLight[i] = 0;
-                if (i < globalCount)
-                {
-                    const float rnd = pre.next(); pre.next(); pre.next(); pre.next();
-                    preLight[i] = __ldg(proxyIndices + min(uint(rnd * float(M)), M - 1));
-                }
-            }
-            #pragma unroll
-            for (uint i = 0; i < kPrefetch; i++)
-                if (i < globalCount)
-                {
-#ifdef __CUDA_ARCH__    // (the host build of tests/emu/shade_host_emu.cu has no PTX)
-                    asm volatile("prefetch.global.L1 [%0];" ::"l"(p.scene.lights + preLight[i]));
-                    asm volatile("prefetch.global.L1 [%0];" ::"l"(proxyCounters + preLight[i]));
-#endif
-                }
+        uint* ctr = nullptr; uint block = 0;
+        if constexpr (MULTI)
+        {   // the vertex's NEE block: header now, one fp32 result per valid sample below
+            ctr = p.wf.counters + p.iteration * kCountersPerIter;
+            block = appendActive(ctr + kCtrNeeBlocks) * (1u + fullSamples);
+            uint choice = 0;
+            if constexpr (kFill) addFillSpecAvgChoice(choice, preFlags, preCounters);
+            p.neeBlocks[block] = make_uint4(slot, choice, 0u, 0u);
         }
-        #pragma unroll 1
-        for (uint i = 0; i < candidateCount; i++)
+        for (uint lightSample = 0; lightSample < (MULTI ? fullSamples : 1u); lightSample++)
         {
-            const float rnd = uniformSG.next();
-            uint lightIndex;
-            switch (i)
-            {   // static indexing keeps preLight[] in registers
-            case 0: lightIndex = preLight[0]; break; case 1: lightIndex = preLight[1]; break; case 2: lightIndex = preLight[2]; break; case 3: lightIndex = preLight[3]; break;
-            case 4: lightIndex = preLight[4]; break; case 5: lightIndex = preLight[5]; break; case 6: lightIndex = preLight[6]; break; case 7: lightIndex = preLight[7]; break;
-            default: lightIndex = proxyIndices[min(uint(rnd * float(M)), M - 1)]; break;
-            }
-            float selectionPdf;
-            const bool sampleIsLocal = NEEAT && i >= globalCount;
-            if (sampleIsLocal) lightIndex = neeat::sampleLocal(p.na, tileAddress, rnd, selectionPdf);
-            else selectionPdf = float(proxyCounters[lightIndex]) / float(M);
-            const LightInfo li = p.scene.lights[lightIndex];
-            const float r0 = uniformSG.next(), r1 = uniformSG.next();
-            float3 lsPos = mk3(0.f), lsRadiance = mk3(0.f); float lsSolidPdf = 0.f; bool lsBsdfSampleable = true;
-            if (ANALYTIC_LIGHTS && lightType(li) == kLightTypeSphere)
-            {   // SphereLight::CalcSample (PolymorphicLight.hlsli:107-181): cone sampling of the visible cap; never found by BSDF rays
-                lsBsdfSampleable = false;
-                sampleSphereLight(li, p.scene, lightIndex, r0, r1, s.posW, lsPos, lsRadiance, lsSolidPdf);
-            }
-            else if (lightType(li) == kLightTypeTriangle)
-            {   // TriangleLight::CalcSample (PolymorphicLight.hlsli:409-441)
-                TriLight tl; tl.decode(li);
-                const float sq = sqrtf(r0);
-                lsPos = offsetRayOrigin(tl.base + tl.e1 * (sq * (1 - r1)) + tl.e2 * (sq * r1), tl.normal);
-                const float3 toLight = lsPos - s.posW;
-                const float dist = sqrtf(fmaxf(2e-9f, dot3(toLight, toLight)));
-                const float cosTheta = dot3(tl.normal, -(toLight / dist));
-                if (cosTheta > 0.f) { lsSolidPdf = fminf(1e10f, pdfAreaToSolidAngle(fmaxf(2e-9f, 1.0f / tl.area), dist, cosTheta)); lsRadiance = tl.radiance; }
-            }
-            else if (lightType(li) == kLightTypeEnvQuad)
-            {   // EnvironmentQuadLight::CalcSample (PolymorphicLight.hlsli:576-599), NEE_AT_SAMPLE_BAKED_ENVIRONMENT
-                const uint nodeX = li.direction1 >> 16, nodeY = li.direction1 & 0xFFFF, nodeDim = li.direction2 >> 16;
-                const float3 worldDir = rowVecTimes3x3(octEqualAreaToDir(mk2((float(nodeX) + r0) / float(nodeDim), (float(nodeY) + r1) / float(nodeDim))), p.c.envMap.Transform);
-                lsPos = s.posW + worldDir * kDistantLightDistance;
-                lsRadiance = unpackLightRadiance(li);
-                lsSolidPdf = float(nodeDim * nodeDim) / (4.0f * kPi);
-            }
-            const float pdf = lsSolidPdf * selectionPdf;
-            const float3 Li = pdf > 0.f ? (lsRadiance / pdf) : mk3(0.f);
-            const float3 surfToLight = lsPos - s.posW;
-            const float dist = len3(surfToLight);
-            const float3 dirToLight = surfToLight / fmaxf(dist, 1e-7f);
-            const float wrsWeight = maxComp(Li) * bsdf.pdf(dirToLight);
-            const float wrsRnd = uniformSG.next();
-            weightSum += wrsWeight;
-            if (wrsRnd < sat(wrsWeight / weightSum)) { pickLi = Li; pickDir = dirToLight; pickDist = dist; pickSelPdf = selectionPdf; pickSolidPdf = lsSolidPdf; pickWeight = wrsWeight; pickBsdfSampleable = lsBsdfSampleable; if (NEEAT) { pickLight = lightIndex; pickLocal = sampleIsLocal; } }
-        }
-        pickLi = pickLi * (1.0f / (pickWeight / weightSum));
-        if (anyPositive(pickLi))
-        {   // ProcessLightSample with visibility deferred to the shadow kernel
-            const float fadeOut = (s.shadowNoLFadeout > 0) ? sat((dot3(pickDir, s.vertexN) - s.shadowNoLFadeout) / (2.0f * s.shadowNoLFadeout)) : 1.0f;
-            // ComputeLightSelectionPdfs: the pdf the other sampler would have picked this light with, and how many candidates this sampler drew
-            float otherPdf = 0.0f, thisCount = float(candidateCount);
-            if constexpr (NEEAT)
+            float3 pickLi = mk3(0.f), pickDir = mk3(0.f); float pickDist = 0.f, pickSelPdf = 0.f, pickSolidPdf = 0.f;
+            float weightSum = 0.f, pickWeight = 0.f; bool pickBsdfSampleable = true;
+            uint pickLight = 0xFFFFFFFFu; bool pickLocal = false;
+            // The candidate loop is a chain of dependent random gathers (proxy table -> counter, light record).  The light selection draws are
+            // every 4th value of the stream, so the proxy lookups of the first 8 candidates are issued up front and their light records
+            // prefetched into L2/L1 before the loop consumes them one by one.
+            constexpr uint kPrefetch = 8;
+            uint preLight[kPrefetch];
             {
-                thisCount = float(globalCount);
-                if (pickLocal) { otherPdf = naGlobalLightPdf(p, pickLight); thisCount = float(localCount); }
-                else if (localCount != 0) otherPdf = neeat::sampleLocalPdf(p.na, tileAddress, pickLight);
-            }
-            const float wrsMIS = misBalance(pickSelPdf, otherPdf) / thisCount;             // without feedback all candidates come from the global table
-            const float scatterPdfForDir = bsdf.pdf(pickDir);
-            const float pathMIS = misBalance((pickSelPdf + otherPdf) * float(fullSamples) * pickSolidPdf, pickBsdfSampleable ? scatterPdfForDir : 0.0f);    // LightSampleableByBSDF
-            const float3 Li = pickLi * (fadeOut * wrsMIS * pathMIS / float(fullSamples));
-            const float4 bsdfThp = bsdf.eval(pickDir);
-            float3 radiance = mk3(bsdfThp.x, bsdfThp.y, bsdfThp.z) * Li;
-            const float radianceAvg = average(radiance);
-            float specAvg = bsdfThp.w * average(Li);
-            if (p.c.fireflyFilterThreshold != 0)
-            {
-                const float k = newFireflyK(preFireflyK, pickSelPdf * pickSolidPdf, 1.0f);
-                const float thr = p.c.fireflyFilterThreshold * k;
-                radiance = radiance * ((radianceAvg > thr) ? (1.0f / radianceAvg * thr) : 1.0f);
-            }
-            radiance = radiance * preThp;
-            specAvg *= average(preThp);
-            if constexpr (NEEAT)
-            {   // InsertFeedbackFromNEE's weight (un-filtered radiance x path throughput, biased towards globally improbable lights), inserted by the shadow kernel if visible
-                naFeedback = pickLight | (isSSC ? 0x80000000u : 0u);
-                naFeedbackWeight = __fdiv_rn(radianceAvg * average(preThp), powf(naGlobalLightPdf(p, pickLight), 0.65f));
-            }
-            const float faceSide = dot3(s.N, pickDir) >= 0 ? 1.0f : -1.0f;
-            const float3 o = offsetRayOrigin(s.posW, s.faceN * faceSide);
-            out.emitShadow = true;
-            out.shadow.originTMax = make_float4(o.x, o.y, o.z, pickDist * 0.9985f);
-            out.shadow.dirPath = make_float4(pickDir.x, pickDir.y, pickDir.z, __uint_as_float(slot));
-            out.shadow.radiance = make_uint2(packHalf2Clamp(radiance.x, radiance.y), packHalf2Clamp(radiance.z, specAvg));   // NEEResult::AccumulateRadiance(0 + x)
-            if constexpr (kFill)
-            {   // which specular average the shadow kernel adds with the radiance (PathTracer.hlsli:731-743); the halves are non-negative, so the sign bits
-                // of the first word carry the choice: 00 none (base scatter was diffuse), 01 the NEE result's own, 10 the whole radiance
-                if (!(preFlags & (kPFStablePlaneBaseScatterDiff << kVertexIndexBits)))
+                UniformSeq pre = uniformSG;
+                #pragma unroll
+                for (uint i = 0; i < kPrefetch; i++)
                 {
-                    const uint bouncesFromStablePlane = ((preCounters >> (kCtrBouncesFromStablePlane << 3)) & 0xffu) + 1u;
-                    const bool special = (bouncesFromStablePlane == 1) || ((preFlags & (kPFDeltaOnlyPath << kVertexIndexBits)) && bouncesFromStablePlane <= 3);
-                    out.shadow.radiance.x |= special ? 0x00008000u : 0x80000000u;
+                    preLight[i] = 0;
+                    if (i < globalCount)
+                    {
+                        const float rnd = pre.next(); pre.next(); pre.next(); pre.next();
+                        preLight[i] = __ldg(proxyIndices + min(uint(rnd * float(M)), M - 1));
+                    }
+                }
+                #pragma unroll
+                for (uint i = 0; i < kPrefetch; i++)
+                    if (i < globalCount)
+                    {
+    #ifdef __CUDA_ARCH__    // (the host build of tests/emu/shade_host_emu.cu has no PTX)
+                        asm volatile("prefetch.global.L1 [%0];" ::"l"(p.scene.lights + preLight[i]));
+                        asm volatile("prefetch.global.L1 [%0];" ::"l"(proxyCounters + preLight[i]));
+    #endif
+                    }
+            }
+            #pragma unroll 1
+            for (uint i = 0; i < candidateCount; i++)
+            {
+                const float rnd = uniformSG.next();
+                uint lightIndex;
+                switch (i)
+                {   // static indexing keeps preLight[] in registers
+                case 0: lightIndex = preLight[0]; break; case 1: lightIndex = preLight[1]; break; case 2: lightIndex = preLight[2]; break; case 3: lightIndex = preLight[3]; break;
+                case 4: lightIndex = preLight[4]; break; case 5: lightIndex = preLight[5]; break; case 6: lightIndex = preLight[6]; break; case 7: lightIndex = preLight[7]; break;
+                default: lightIndex = proxyIndices[min(uint(rnd * float(M)), M - 1)]; break;
+                }
+                float selectionPdf;
+                const bool sampleIsLocal = NEEAT && i >= globalCount;
+                if (sampleIsLocal) lightIndex = neeat::sampleLocal(p.na, tileAddress, rnd, selectionPdf);
+                else selectionPdf = float(proxyCounters[lightIndex]) / float(M);
+                const LightInfo li = p.scene.lights[lightIndex];
+                const float r0 = uniformSG.next(), r1 = uniformSG.next();
+                float3 lsPos = mk3(0.f), lsRadiance = mk3(0.f); float lsSolidPdf = 0.f; bool lsBsdfSampleable = true;
+                if (ANALYTIC_LIGHTS && lightType(li) == kLightTypeSphere)
+                {   // SphereLight::CalcSample (PolymorphicLight.hlsli:107-181): cone sampling of the visible cap; never found by BSDF rays
+                    lsBsdfSampleable = false;
+                    sampleSphereLight(li, p.scene, lightIndex, r0, r1, s.posW, lsPos, lsRadiance, lsSolidPdf);
+                }
+                else if (lightType(li) == kLightTypeTriangle)
+                {   // TriangleLight::CalcSample (PolymorphicLight.hlsli:409-441)
+                    TriLight tl; tl.decode(li);
+                    const float sq = sqrtf(r0);
+                    lsPos = offsetRayOrigin(tl.base + tl.e1 * (sq * (1 - r1)) + tl.e2 * (sq * r1), tl.normal);
+                    const float3 toLight = lsPos - s.posW;
+                    const float dist = sqrtf(fmaxf(2e-9f, dot3(toLight, toLight)));
+                    const float cosTheta = dot3(tl.normal, -(toLight / dist));
+                    if (cosTheta > 0.f) { lsSolidPdf = fminf(1e10f, pdfAreaToSolidAngle(fmaxf(2e-9f, 1.0f / tl.area), dist, cosTheta)); lsRadiance = tl.radiance; }
+                }
+                else if (lightType(li) == kLightTypeEnvQuad)
+                {   // EnvironmentQuadLight::CalcSample (PolymorphicLight.hlsli:576-599), NEE_AT_SAMPLE_BAKED_ENVIRONMENT
+                    const uint nodeX = li.direction1 >> 16, nodeY = li.direction1 & 0xFFFF, nodeDim = li.direction2 >> 16;
+                    const float3 worldDir = rowVecTimes3x3(octEqualAreaToDir(mk2((float(nodeX) + r0) / float(nodeDim), (float(nodeY) + r1) / float(nodeDim))), p.c.envMap.Transform);
+                    lsPos = s.posW + worldDir * kDistantLightDistance;
+                    lsRadiance = unpackLightRadiance(li);
+                    lsSolidPdf = float(nodeDim * nodeDim) / (4.0f * kPi);
+                }
+                const float pdf = lsSolidPdf * selectionPdf;
+                const float3 Li = pdf > 0.f ? (lsRadiance / pdf) : mk3(0.f);
+                const float3 surfToLight = lsPos - s.posW;
+                const float dist = len3(surfToLight);
+                const float3 dirToLight = surfToLight / fmaxf(dist, 1e-7f);
+                const float wrsWeight = maxComp(Li) * bsdf.pdf(dirToLight);
+                const float wrsRnd = uniformSG.next();
+                weightSum += wrsWeight;
+                if (wrsRnd < sat(wrsWeight / weightSum)) { pickLi = Li; pickDir = dirToLight; pickDist = dist; pickSelPdf = selectionPdf; pickSolidPdf = lsSolidPdf; pickWeight = wrsWeight; pickBsdfSampleable = lsBsdfSampleable; if (NEEAT) { pickLight = lightIndex; pickLocal = sampleIsLocal; } }
+            }
+            pickLi = pickLi * (1.0f / (pickWeight / weightSum));
+            if (anyPositive(pickLi))
+            {   // ProcessLightSample with visibility deferred to the shadow kernel
+                const float fadeOut = (s.shadowNoLFadeout > 0) ? sat((dot3(pickDir, s.vertexN) - s.shadowNoLFadeout) / (2.0f * s.shadowNoLFadeout)) : 1.0f;
+                // ComputeLightSelectionPdfs: the pdf the other sampler would have picked this light with, and how many candidates this sampler drew
+                float otherPdf = 0.0f, thisCount = float(candidateCount);
+                if constexpr (NEEAT)
+                {
+                    thisCount = float(globalCount);
+                    if (pickLocal) { otherPdf = naGlobalLightPdf(p, pickLight); thisCount = float(localCount); }
+                    else if (localCount != 0) otherPdf = neeat::sampleLocalPdf(p.na, tileAddress, pickLight);
+                }
+                const float wrsMIS = misBalance(pickSelPdf, otherPdf) / thisCount;             // without feedback all candidates come from the global table
+                const float scatterPdfForDir = bsdf.pdf(pickDir);
+                const float pathMIS = misBalance((pickSelPdf + otherPdf) * float(fullSamples) * pickSolidPdf, pickBsdfSampleable ? scatterPdfForDir : 0.0f);    // LightSampleableByBSDF
+                const float3 Li = pickLi * (fadeOut * wrsMIS * pathMIS / float(fullSamples));
+                const float4 bsdfThp = bsdf.eval(pickDir);
+                float3 radiance = mk3(bsdfThp.x, bsdfThp.y, bsdfThp.z) * Li;
+                const float radianceAvg = average(radiance);
+                float specAvg = bsdfThp.w * average(Li);
+                if (p.c.fireflyFilterThreshold != 0)
+                {
+                    const float k = newFireflyK(preFireflyK, pickSelPdf * pickSolidPdf, 1.0f);
+                    const float thr = p.c.fireflyFilterThreshold * k;
+                    radiance = radiance * ((radianceAvg > thr) ? (1.0f / radianceAvg * thr) : 1.0f);
+                }
+                radiance = radiance * preThp;
+                specAvg *= average(preThp);
+                if constexpr (NEEAT)
+                {   // InsertFeedbackFromNEE's weight (un-filtered radiance x path throughput, biased towards globally improbable lights), inserted by the shadow kernel if visible
+                    naFeedback = pickLight | (isSSC ? 0x80000000u : 0u);
+                    naFeedbackWeight = __fdiv_rn(radianceAvg * average(preThp), powf(naGlobalLightPdf(p, pickLight), 0.65f));
+                }
+                const float faceSide = dot3(s.N, pickDir) >= 0 ? 1.0f : -1.0f;
+                const float3 o = offsetRayOrigin(s.posW, s.faceN * faceSide);
+                if constexpr (MULTI)
+                {   // this sample's shadow record (long rays first, as appendShadowRecord) and its result, which k_nee_resolve adds if the shadow kernel marks it visible
+                    const uint e = appendShadowRecordActive(p, ctr, pickDist * 0.9985f, neeShadowCapacity(p));
+                    p.wf.shadowOriginTMax[e] = make_float4(o.x, o.y, o.z, pickDist * 0.9985f);
+                    p.wf.shadowDirPath[e] = make_float4(pickDir.x, pickDir.y, pickDir.z, __uint_as_float(block));
+                    p.wf.shadowRadiance[e] = make_uint2(lightSample, 0u);
+                    p.neeBlocks[block + 1u + lightSample] = make_uint4(__float_as_uint(radiance.x), __float_as_uint(radiance.y), __float_as_uint(radiance.z), __float_as_uint(specAvg));
+                }
+                else
+                {
+                    out.emitShadow = true;
+                    out.shadow.originTMax = make_float4(o.x, o.y, o.z, pickDist * 0.9985f);
+                    out.shadow.dirPath = make_float4(pickDir.x, pickDir.y, pickDir.z, __uint_as_float(slot));
+                    out.shadow.radiance = make_uint2(packHalf2Clamp(radiance.x, radiance.y), packHalf2Clamp(radiance.z, specAvg));   // NEEResult::AccumulateRadiance(0 + x)
+                    if constexpr (kFill) addFillSpecAvgChoice(out.shadow.radiance.x, preFlags, preCounters);     // the specular average the shadow kernel adds with the radiance
                 }
             }
         }

@@ -38,7 +38,8 @@ __global__ void k_init_sobol_tables()
 void launchInitTables(cudaStream_t s) { k_init_sobol_tables<<<16, 256, 0, s>>>(); }
 
 // ---- shade --------------------------------------------------------------------------------------------------------------------------------
-template <int MINB, bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, bool NEEAT = false>
+// MULTI (NEEFullSamples > 1): shadeHit appends the vertex's shadow records and NEE block itself, one record per valid light sample
+template <int MINB, bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false>
 __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
@@ -61,7 +62,7 @@ __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ Lau
                 h = path.loadRay(p.stateIn, r, p.radiance);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
                 if (cls == 0) shadeMiss<EXPORT_GUIDES, kModeReference, NEEAT>(p, path);
-                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT>(p, path, h, p.wf.hits[r], out);
+                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT, MULTI>(p, path, h, p.wf.hits[r], out);
                 path.storeRadiance(p.radiance, h);
                 if (out.continuePath) rayCls = 0;
                 if (out.emitShadow) shadowCls = 0;
@@ -70,6 +71,7 @@ __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ Lau
             const uint next = warpAppend(ctrNext + kCtrRayCount, rayCls);
             if (rayCls == 0) path.storeRay(p.stateOut, next, h);
             // shadow records: warp-aggregated, long rays from the front of the three arrays, the rest from the back (appendShadowRecord)
+            if constexpr (!MULTI)
             {
                 const uint b = appendShadowRecord(p, ctr, shadowCls == 0, out.shadow.originTMax.w);
                 if (shadowCls == 0)
@@ -115,6 +117,11 @@ void launchShade(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
 {
     const int grid = g.smCount * g.shadeBlocksPerSM;
     // guide export and analytic (sphere) lights are separate instantiations: the default kernel carries neither
+    if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1)
+    {   // several light samples per vertex: analytic lights compiled in, gated by the light type at run time
+        if (p.exportGuides) k_shade<3, true, true, false, true><<<g.smCount * 3, 128, 0, s>>>(p); else k_shade<3, false, true, false, true><<<g.smCount * 3, 128, 0, s>>>(p);
+        return;
+    }
     if (p.exportGuides) { k_shade<4, true, true><<<g.smCount * 4, 128, 0, s>>>(p); return; }
     if (p.scene.analyticLightCount != 0) { k_shade<4, false, true><<<g.smCount * 4, 128, 0, s>>>(p); return; }
     if (g.shadeBlocksPerSM >= 5) k_shade<5, false, false><<<grid, 128, 0, s>>>(p);

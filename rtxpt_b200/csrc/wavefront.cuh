@@ -58,7 +58,8 @@ constexpr int kCtrShadowTriTests = kCtrShadowNodeVisits + 1;
 constexpr int kCtrFetchClosest = kCtrShadowTriTests + 1;    // dynamic ray fetch cursors of the persistent traversal warps
 constexpr int kCtrFetchShadow = kCtrFetchClosest + 1;
 constexpr int kCtrShadowShort = kCtrFetchShadow + 1;        // shadow records appended from the END of the record arrays (see appendShadowRecord); kCtrShadowCount counts the ones at the front
-static_assert(kCtrShadowShort < 20, "counter block");
+constexpr int kCtrNeeBlocks = kCtrShadowShort + 1;          // NEE blocks appended by a multi-sample shade (NEEFullSamples > 1, see NEE blocks below)
+static_assert(kCtrNeeBlocks < 20, "counter block");
 constexpr int kCountersPerIter = 20;
 
 // realtime mode (stable planes): the reference's u_StablePlanesHeader / u_StablePlanesBuffer / u_StableRadiance / u_SpecularHitT and the
@@ -111,13 +112,103 @@ struct LaunchParams
     RealtimeParams rt;
     // NEE-AT temporal feedback (kernels instantiated with NEEAT = true only; appended so that every other kernel's parameter offsets stay what they were)
     neeat::Params na;
-    uint4* naShadowFeedback;        // per shadow record: light | ssc << 31, feedback weight, reservoir random, Russian roulette outcome had the sample been visible
+    union
+    {
+        uint4* naShadowFeedback;    // per shadow record: light | ssc << 31, feedback weight, reservoir random, Russian roulette outcome had the sample been visible
+        uint4* neeBlocks;           // NEEFullSamples > 1 (multi-sample kernels, which never run with feedback): the NEE blocks (see below)
+    };
     uint* naRrFix;                  // per home index h: set by the shadow kernel when the sample was visible, consumed by the next shade of the path
     // reference mode's ray-ordered state (see the top of this file; appended for the same reason): the set this iteration's rays are read from,
     // the set its continuing paths are appended to, and the radiance per home index h
     StateSet stateIn, stateOut;
     uint2* radiance;
 };
+static_assert(sizeof(LaunchParams) == 1632, "the parameter block of every kernel keeps its layout");
+
+// ---- NEE blocks (NEEFullSamples = N > 1) ---------------------------------------------------------------------------------------------------------------
+// A vertex that takes light samples appends one block of 1 + N uint4 (counter kCtrNeeBlocks) to LaunchParams::neeBlocks: a header { path slot or home index h, the FILL
+// pass's specular-average choice bits (shade.cuh), visibility mask bits 0..31, bits 32..63 } and per sample j the fp32 (radiance.rgb, specAvg) it adds if visible.  The
+// shadow-record arrays then hold up to N records per path: sample j's record carries the header's index in dirPath.w and j in radiance.x; the shadow kernel sets bit j
+// of the mask when the light is visible, and k_nee_resolve sums the block.
+constexpr uint kNeeMaxFullSamples = 63;         // min( 63, NEEFullSamples ), PathTracerNEE.hlsli:306
+PT_HD uint neeShadowCapacity(const LaunchParams& p) { return p.wf.capacity * min(kNeeMaxFullSamples, p.c.NEEFullSamples); }      // length of the shadow-record arrays
+
+// warp-aggregated append of one entry per calling lane among the lanes that are active together (the multi-sample shade appends from inside its divergent sample loop)
+PT_DEVICE uint appendActive(uint* ctr)
+{
+#ifdef __CUDA_ARCH__
+    const uint active = __activemask(), lane = threadIdx.x & 31u, leader = __ffs(active) - 1u;
+    uint base = 0;
+    if (lane == leader) base = atomicAdd(ctr, __popc(active));
+    return __shfl_sync(active, base, leader) + __popc(active & ((1u << lane) - 1u));
+#else
+    return atomicAdd(ctr, 1u);      // host build of the shading functions (tests/emu): one lane
+#endif
+}
+// appendShadowRecord for the lanes that are active together, every one of which emits a record; `capacity` is the length of the record arrays
+PT_DEVICE uint appendShadowRecordActive(const LaunchParams& p, uint* ctr, float tMax, uint capacity)
+{
+    const bool isLong = tMax > p.shadowLongRayT;
+#ifdef __CUDA_ARCH__
+    const uint active = __activemask(), lane = threadIdx.x & 31u;
+    const uint longPeers = __ballot_sync(active, isLong), peers = isLong ? longPeers : (active & ~longPeers), leader = __ffs(peers) - 1u;
+    uint base = 0;
+    if (lane == leader) base = atomicAdd(ctr + (isLong ? kCtrShadowCount : kCtrShadowShort), __popc(peers));
+    base = __shfl_sync(active, base, leader) + __popc(peers & ((1u << lane) - 1u));
+#else
+    const uint base = atomicAdd(ctr + (isLong ? kCtrShadowCount : kCtrShadowShort), 1u);
+#endif
+    return isLong ? base : capacity - 1u - base;
+}
+
+// What HandleHit does with a vertex's NEE result once visibility is known (PathTracer.hlsli:725-746): if any half of the packed (radiance, specAvg) is positive,
+// AccumulatePathRadiance.  REALTIME (FILL pass): attenuated by 1 / sub-sample count, with the specular average chosen by the sign bits of r.x (shadeHit); reference mode:
+// `slot` is the path's home index h.  The shadow kernel applies a single sample's record with it, k_nee_resolve the sum of a block.
+template <bool REALTIME>
+PT_DEVICE void accumulateNeeRadiance(const LaunchParams& p, uint slot, uint2 r)
+{
+    const float rx = f16tof32(r.x & 0x7FFFu), ry = f16tof32((r.x >> 16) & 0x7FFFu), rz = f16tof32(r.y), rw = f16tof32(r.y >> 16);
+    if (rx > 0 || ry > 0 || rz > 0 || rw > 0)
+    {
+        if constexpr (REALTIME)
+        {
+            uint4 s2 = p.wf.s2[slot];
+            const float a = p.rt.attenuation;
+            const float spec = (r.x & 0x00008000u) ? rw : ((r.x & 0x80000000u) ? (rx + ry + rz) / 3.0f : 0.0f);
+            const float lx = f16tof32(s2.z) + rx * a, ly = f16tof32(s2.z >> 16) + ry * a, lz = f16tof32(s2.w) + rz * a, lw = f16tof32(s2.w >> 16) + spec * a;
+            s2.z = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
+            s2.w = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
+            p.wf.s2[slot] = s2;
+        }
+        else
+        {
+            uint2 l = p.radiance[slot];
+            const float lx = f16tof32(l.x) + rx, ly = f16tof32(l.x >> 16) + ry, lz = f16tof32(l.y) + rz, lw = f16tof32(l.y >> 16);
+            l.x = packHalf2NoClamp(clampf(lx, 0.f, kHalfMax), clampf(ly, 0.f, kHalfMax));
+            l.y = packHalf2NoClamp(clampf(lz, 0.f, kHalfMax), clampf(lw, 0.f, kHalfMax));
+            p.radiance[slot] = l;
+        }
+    }
+}
+
+// k_nee_resolve's body for the block at `block`: the visible samples summed in sample order as NEEResult::AccumulateRadiance does - each fp32 term added to the fp32 value
+// of the running fp16 sum, which is rounded back to fp16 after every sample (PathTracerNEE.hlsli:277-346) - then applied once, as the shadow kernel applies one record
+template <bool REALTIME>
+PT_DEVICE void resolveNeeBlock(const LaunchParams& p, const uint4* block)
+{
+    const uint4 h = block[0];
+    uint2 sum = make_uint2(0u, 0u);
+    for (uint j = 0; j <= kNeeMaxFullSamples; j++)
+    {
+        const uint bit = j < 32 ? (h.z >> j) & 1u : (h.w >> (j - 32)) & 1u;
+        if (!bit) continue;
+        const uint4 s = block[1 + j];
+        sum.x = packHalf2Clamp(f16tof32(sum.x) + __uint_as_float(s.x), f16tof32(sum.x >> 16) + __uint_as_float(s.y));
+        sum.y = packHalf2Clamp(f16tof32(sum.y) + __uint_as_float(s.z), f16tof32(sum.y >> 16) + __uint_as_float(s.w));
+    }
+    sum.x |= h.y;
+    accumulateNeeRadiance<REALTIME>(p, h.x, sum);
+}
 
 // every lane of the warp calls this; `emit` lanes get the index of their shadow record
 PT_DEVICE uint appendShadowRecord(const LaunchParams& p, uint* ctr, bool emit, float tMax)
