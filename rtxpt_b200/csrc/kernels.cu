@@ -89,8 +89,9 @@ constexpr uint kTraceScratchBytes = 16 + kTraceWarps * sizeof(WarpScratch);
 //   fetchRay(i, o, d, tMin, tMax)  loads ray i and keeps what the caller needs when the ray retires
 //   retireRay(retireMask, ws)      called by every lane whose ray has finished, with its result in ws (Traverser::result); with RETIRE_MASK
 //                                  retireMask is the ballot of those lanes, for warp-collective work among them (0 otherwise: no vote is taken)
+// TMIN_ZERO: fetchRay gives every ray tMin == 0, which lets the node step compare distances as integers (traverse.cuh: nodeHitMask).
 // Returns this thread's traversal counters (zero unless COUNT).
-template <bool ANY_HIT, bool COUNT, bool RETIRE_MASK, typename FetchRay, typename RetireRay>
+template <bool ANY_HIT, bool COUNT, bool RETIRE_MASK, bool TMIN_ZERO, typename FetchRay, typename RetireRay>
 PT_DEVICE TraversalCounters traceLoop(const LaunchParams& p, uint* fetchCursor, uint count, FetchRay&& fetchRay, RetireRay&& retireRay)
 {
     extern __shared__ __align__(16) unsigned char smemRaw[];
@@ -101,7 +102,7 @@ PT_DEVICE TraversalCounters traceLoop(const LaunchParams& p, uint* fetchCursor, 
 
     TraversalCounters tc; tc.nodeVisits = 0; tc.triTests = 0;
     const uint lane = threadIdx.x & 31u, laneLt = (1u << lane) - 1u;
-    Traverser<ANY_HIT, COUNT> tv; tv.done = true; tv.waiting = false;
+    Traverser<ANY_HIT, COUNT, TMIN_ZERO> tv; tv.done = true; tv.waiting = false;
     uint2 stack[kTraversalStackSize];
     uint head = 0, tail = 0;
     if (lane == 0) ws.tail = 0;
@@ -178,7 +179,7 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
     {   // hit record + SER-style binning by {miss, terminating hit, material class}
         const uint lane = threadIdx.x & 31u, laneLt = (1u << lane) - 1u;
         const uint slot = entry & 0x7FFFFFFFu;
-        uint subInstance; const HitRecord h = Traverser<false, COUNT>::result(ws, subInstance);
+        uint subInstance; const HitRecord h = Traverser<false, COUNT, true>::result(ws, subInstance);
         p.wf.hits[slot] = make_float4(h.t, h.u, h.v, __uint_as_float(h.gid));
         uint cls;
         if (h.gid == 0xFFFFFFFFu) cls = 0;
@@ -191,7 +192,7 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
         base = __shfl_sync(peers, base, leader);
         p.wf.shadeQueue[size_t(cls) * p.wf.capacity + base + __popc(peers & laneLt)] = slot;
     };
-    const TraversalCounters tc = traceLoop<false, COUNT, true>(p, ctr + kCtrFetchClosest, count, fetchRay, retireRay);
+    const TraversalCounters tc = traceLoop<false, COUNT, true, true>(p, ctr + kCtrFetchClosest, count, fetchRay, retireRay);
     if (COUNT) { atomicAdd(ctr + kCtrNodeVisits, tc.nodeVisits); atomicAdd(ctr + kCtrTriTests, tc.triTests); }
 }
 
@@ -233,7 +234,7 @@ __global__ void __launch_bounds__(kTraceThreads, MINB * kTraceCtaScale) k_trace_
         }
         visibleCount++;
     };
-    const TraversalCounters tc = traceLoop<true, COUNT, false>(p, ctr + kCtrFetchShadow, count, fetchRay, retireRay);
+    const TraversalCounters tc = traceLoop<true, COUNT, false, true>(p, ctr + kCtrFetchShadow, count, fetchRay, retireRay);
     if (COUNT) { atomicAdd(ctr + kCtrShadowNodeVisits, tc.nodeVisits); atomicAdd(ctr + kCtrShadowTriTests, tc.triTests); atomicAdd(ctr + kCtrShadowVisible, visibleCount); }
 }
 
@@ -289,13 +290,13 @@ __global__ void __launch_bounds__(kTraceThreads, 2 * kTraceCtaScale) k_trace_ray
     };
     auto retireRay = [&](uint, const WarpScratch& ws)
     {
-        uint subInstance; const HitRecord h = Traverser<ANY_HIT, true>::result(ws, subInstance);
+        uint subInstance; const HitRecord h = Traverser<ANY_HIT, true, false>::result(ws, subInstance);
         RtxptHit r;
         if (h.gid != 0xFFFFFFFFu) { const uint4 info = p.scene.triInfo[h.gid]; r.t = h.t; r.u = h.u; r.v = h.v; r.instanceIndex = info.x; r.geometryIndex = info.y; r.primitiveIndex = info.z; }
         else { r.t = -1.0f; r.u = r.v = 0.f; r.instanceIndex = r.geometryIndex = r.primitiveIndex = 0xFFFFFFFFu; }
         out[index] = r;
     };
-    const TraversalCounters tc = traceLoop<ANY_HIT, true, false>(p, cursor, count, fetchRay, retireRay);
+    const TraversalCounters tc = traceLoop<ANY_HIT, true, false, false>(p, cursor, count, fetchRay, retireRay);
     if (counters) { atomicAdd(counters + 0, tc.nodeVisits); atomicAdd(counters + 1, tc.triTests); }
 }
 

@@ -112,15 +112,24 @@ __device__ __noinline__ bool alphaCandidateIsOpaque(const SceneView& sc, uint su
 struct TraversalCounters { uint nodeVisits, triTests; };
 
 // byte j of a packed word -> 1 + b * 2^-15, built by placing the byte in mantissa bits 8..15 of 1.0f (one PRMT)
-PT_DEVICE float byteToUnitFloat(uint w, int j) { return __uint_as_float(__byte_perm(w, 0x3F800000u, 0x7604u | (uint(j) << 4))); }
+PT_HD float byteToUnitFloat(uint w, int j)
+{
+#ifdef __CUDA_ARCH__
+    return __uint_as_float(__byte_perm(w, 0x3F800000u, 0x7604u | (uint(j) << 4)));
+#else
+    return bitsToFloat(0x3F800000u | (((w >> (8 * j)) & 0xFFu) << 8));
+#endif
+}
 #ifndef PT_I2F_AXES
 #define PT_I2F_AXES 2       // how many of the three axes convert their bytes with I2F (XU pipe) instead of PRMT (ALU pipe): 2 spreads the conversions over both pipes.
-                            // H100 SXM (700 W), bench.py ms/frame: 1 axis 23.50, 2 axes 23.16-23.18, 3 axes 23.59
+                            // H100 80GB HBM3 (700 W, 1980 MHz), bench.py ms/frame, three alternating runs each (scripts/bench_slab_ab.py), with the integer slab compare:
+                            // 1 axis 20.86-20.98, 2 axes 20.68-20.72 (and one run at 21.25), 3 axes 21.42-21.50
 #endif
 // the same permute with the selector as an immediate: `one` is 0x3F800000 held in a register the compiler cannot see through (otherwise ptxas folds it into the
 // instruction's only immediate slot and spends a second instruction per byte on moving the selector into a register - 16 per node visit in the round-1 SASS)
-PT_DEVICE float byteToUnitFloatImm(uint w, int j, uint one)
+PT_HD float byteToUnitFloatImm(uint w, int j, uint one)
 {
+#ifdef __CUDA_ARCH__
     uint r;
     switch (j)
     {
@@ -130,11 +139,111 @@ PT_DEVICE float byteToUnitFloatImm(uint w, int j, uint one)
     default: asm("prmt.b32 %0, %1, %2, 0x7634;" : "=r"(r) : "r"(w), "r"(one)); break;
     }
     return __uint_as_float(r);
+#else
+    return byteToUnitFloat(w, j);
+#endif
 }
 #ifndef PT_PRMT_IMM
 #define PT_PRMT_IMM 0      // immediate PRMT selectors: the saved selector moves are re-spent on re-materialising the constant (H100 SXM, 700 W, bench.py: 23.27 ms/frame with, 23.16-23.18 without)
 #endif
-template <bool I2F> PT_DEVICE float byteToCoord(uint w, int j, uint one) { return I2F ? float((w >> (8 * j)) & 0xFFu) : (PT_PRMT_IMM ? byteToUnitFloatImm(w, j, one) : byteToUnitFloat(w, j)); }
+template <bool I2F> PT_HD float byteToCoord(uint w, int j, uint one) { return I2F ? float((w >> (8 * j)) & 0xFFu) : (PT_PRMT_IMM ? byteToUnitFloatImm(w, j, one) : byteToUnitFloat(w, j)); }
+PT_HD uint byteOf(uint w, int j)
+{
+#ifdef __CUDA_ARCH__
+    return __byte_perm(w, 0u, 0x4440u | uint(j));
+#else
+    return (w >> (8 * j)) & 0xFFu;
+#endif
+}
+PT_HD float fmaRn(float a, float b, float c)
+{
+#ifdef __CUDA_ARCH__
+    return __fmaf_rn(a, b, c);
+#else
+    return fmaf(a, b, c);
+#endif
+}
+
+// ---- node step -------------------------------------------------------------------------------------------------------------------------------
+// One ray against the eight quantised child boxes of one CWBVH8 node (n0..n4: its five 16-byte words).  Returns the node's hit word in traversal order: bits 24..31 the inner
+// children the ray enters (the bit index of slot s is 24 + (s ^ octinv), so the highest set bit is the nearest octant), bits 0..23 the triangles of the leaf children it enters.
+// org, idx/idy/idz (reciprocal direction) and octinv are the ray's constants (Traverser::init); the ray's interval is [tMin, bestT].
+// __host__ __device__ so that tests/emu can run it on the CPU against the formulation it replaced (tests/test_slab_compare_port.py).
+//
+// Slab test.  A quantised coordinate byte b is turned into the float m = 1 + b * 2^-15 with one byte permute (ALU pipe) instead of an integer->float conversion (quarter-rate
+// XU pipe, the top pipe of this kernel in the round-1 ncu capture); then b * (s * id) + o == m * A + (o - A) with A = s * id * 2^15.  The box test only has to be conservative
+// (the triangle test decides): the relative slack eps and an absolute pad that covers the rounding of (o - A) (<= 2^-22 (|A| + |o|), |o| <= |t| + 2^8 |s id|) are folded into
+// the per-node constants, near planes pulled in, far pushed out.  PT_I2F_AXES of the three axes keep the integer->float conversion (XU pipe) so that the conversions are spread
+// over two pipes: for those, b * (s id) + o is evaluated directly (A = s id, no offset), with the same slack.
+//
+// TMIN_ZERO (every ray of the wavefront: tMin is 0 by construction, and it is not read): the six plane distances are compared as the signed integers their bit patterns are, with
+// sm_90's three-input integer min / max (VIMNMX3, the DPX instructions) - four ALU-pipe instructions per child where the float form takes seven FMNMX / FSETP.  The outcome is the
+// float one:
+//   * non-negative floats order like their bit patterns and every negative float is a negative integer, so max(t0x, t0y, t0z, 0) - the .RELU form clamps at zero - is exact;
+//   * if every far distance is >= 0 the integer minimum is the float minimum; if one is negative the integer minimum is negative (not necessarily the same one), and the child is
+//     rejected either way, because cmin >= 0.  -0 is INT_MIN: a far distance of -0 is rejected where the float compare 0 <= -0 accepts.  That is as conservative (no t > 0
+//     lies in such a box), and a fused m * A + O is -0 only if the product is a zero, i.e. A == 0, which a finite non-zero idx and the builder's scales exclude.
+//   * no NaN reaches the compare, which matters because fmaxf / fminf drop a NaN operand and integers do not: A and O are finite - |idx| <= 1e20 (eps in Traverser::init), the
+//     builder keeps the scale exponent e + 15 < 255, and a scene's |p - org| * |idx| and s * |idx| * 2^15 stay far below FLT_MAX - and m * A + O of finite terms that does
+//     not overflow is not NaN.  (A ray that is NaN itself still ends: whatever its compares answer, the tree is finite and no node is entered twice.)
+// Without TMIN_ZERO (k_trace_rays: callers may pass any tMin, negative included, and then a box behind the origin has to be entered) the comparison stays in floating point.
+template <bool TMIN_ZERO>
+PT_HD uint nodeHitMask(const uint4 n0, const uint4 n1, const uint4 n2, const uint4 n3, const uint4 n4, float3 org, float idx, float idy, float idz, uint octinv,
+                       float tMin, float bestT, uint one)
+{
+    const bool negx = !(octinv & 4u), negy = !(octinv & 2u), negz = !(octinv & 1u);
+    const float px = bitsToFloat(n0.x), py = bitsToFloat(n0.y), pz = bitsToFloat(n0.z);
+    // quantisation scale 2^(e-127) per axis, times 2^15 (bvh_builder.cpp keeps e + 15 < 255)
+    const float sx15 = bitsToFloat(((n0.w & 0xFFu) + 15u) << 23), sy15 = bitsToFloat((((n0.w >> 8) & 0xFFu) + 15u) << 23), sz15 = bitsToFloat((((n0.w >> 16) & 0xFFu) + 15u) << 23);
+    const float Ax15 = sx15 * idx, Ay15 = sy15 * idy, Az15 = sz15 * idz;
+    const float Ax = (PT_I2F_AXES > 0) ? Ax15 * (1.0f / 32768.0f) : Ax15, Ay = (PT_I2F_AXES > 1) ? Ay15 * (1.0f / 32768.0f) : Ay15, Az = (PT_I2F_AXES > 2) ? Az15 * (1.0f / 32768.0f) : Az15;
+    const float ox = (px - org.x) * idx, oy = (py - org.y) * idy, oz = (pz - org.z) * idz;
+    const float Ox = (PT_I2F_AXES > 0) ? ox : ox - Ax, Oy = (PT_I2F_AXES > 1) ? oy : oy - Ay, Oz = (PT_I2F_AXES > 2) ? oz : oz - Az;
+    const float kLo = 1.0f - 6.0e-7f, kHi = 1.0f + 6.0e-7f, kPad = 4.8e-7f;
+    const float Anx = Ax * kLo, Any = Ay * kLo, Anz = Az * kLo, Afx = Ax * kHi, Afy = Ay * kHi, Afz = Az * kHi;
+    const float Onx = fmaRn(Ox, kLo, -fabsf(Ax15) * kPad), Ony = fmaRn(Oy, kLo, -fabsf(Ay15) * kPad), Onz = fmaRn(Oz, kLo, -fabsf(Az15) * kPad);
+    const float Ofx = fmaRn(Ox, kHi, fabsf(Ax15) * kPad), Ofy = fmaRn(Oy, kHi, fabsf(Ay15) * kPad), Ofz = fmaRn(Oz, kHi, fabsf(Az15) * kPad);
+    const int bestTi = int(floatBits(bestT));
+    uint hitmask = 0;
+    #pragma unroll
+    for (int half = 0; half < 2; half++)
+    {
+        // child metadata, four children per word: byte = leaf ? unary triangle count << 5 | first triangle bit : 0b001 << 5 | 24 + slot; 0 = empty.  A hit child contributes
+        // (byte >> 5) << (bit index), the bit index of an inner child (bits 3 and 4 set) xor-ed with octinv: the xor is done on the four bytes at once and leaves the count bits
+        // alone, so per child one byte extract serves both operands of the shift (which takes its amount modulo 32).
+        const uint meta4 = half ? n1.w : n1.z;
+        const uint isInner4 = ((meta4 & (meta4 << 1)) >> 4) & 0x01010101u;
+        const uint slot4 = meta4 ^ (isInner4 * octinv);
+        const uint qlox = half ? n2.y : n2.x, qloy = half ? n2.w : n2.z, qloz = half ? n3.y : n3.x;
+        const uint qhix = half ? n3.w : n3.z, qhiy = half ? n4.y : n4.x, qhiz = half ? n4.w : n4.z;
+        const uint nearx = negx ? qhix : qlox, farx = negx ? qlox : qhix;
+        const uint neary = negy ? qhiy : qloy, fary = negy ? qloy : qhiy;
+        const uint nearz = negz ? qhiz : qloz, farz = negz ? qloz : qhiz;
+        #pragma unroll
+        for (int j = 0; j < 4; j++)
+        {
+            const float t0x = fmaRn(byteToCoord<(PT_I2F_AXES > 0)>(nearx, j, one), Anx, Onx), t1x = fmaRn(byteToCoord<(PT_I2F_AXES > 0)>(farx, j, one), Afx, Ofx);
+            const float t0y = fmaRn(byteToCoord<(PT_I2F_AXES > 1)>(neary, j, one), Any, Ony), t1y = fmaRn(byteToCoord<(PT_I2F_AXES > 1)>(fary, j, one), Afy, Ofy);
+            const float t0z = fmaRn(byteToCoord<(PT_I2F_AXES > 2)>(nearz, j, one), Anz, Onz), t1z = fmaRn(byteToCoord<(PT_I2F_AXES > 2)>(farz, j, one), Afz, Ofz);
+            bool hit;
+            if (TMIN_ZERO)
+            {
+                const int cmin = __vimax3_s32_relu(int(floatBits(t0x)), int(floatBits(t0y)), int(floatBits(t0z)));
+                const int cmax = min(__vimin3_s32(int(floatBits(t1x)), int(floatBits(t1y)), int(floatBits(t1z))), bestTi);
+                hit = cmin <= cmax;
+            }
+            else
+            {
+                const float cmin = fmaxf(fmaxf(t0x, t0y), fmaxf(t0z, tMin));
+                const float cmax = fminf(fminf(t1x, t1y), fminf(t1z, bestT));
+                hit = cmin <= cmax;
+            }
+            const uint m = byteOf(slot4, j);
+            if (hit) hitmask |= (m >> 5) << (m & 31u);
+        }
+    }
+    return hitmask;
+}
 
 // ---- warp-cooperative traversal ------------------------------------------------------------------------------------------------------
 // Node steps are per-lane work (each lane walks its own ray through the CWBVH8).  Triangle tests are NOT: a leaf holds 1..3 triangles and
@@ -165,7 +274,7 @@ static_assert(sizeof(WarpScratch) == 2320, "WarpScratch layout");
 // unfinished ray until fewer than `minActiveLanes` of them are left, so that the caller can fetch new rays for the idle lanes (dynamic
 // fetch, Aila & Laine HPG 2009).  The traversal stack is a separate local array owned by the kernel so that the scalar state stays in
 // registers; head/tail are the warp-uniform ring cursors.
-template <bool ANY_HIT, bool COUNT>
+template <bool ANY_HIT, bool COUNT, bool TMIN_ZERO>
 struct Traverser
 {
     float3 org;
@@ -252,8 +361,6 @@ struct Traverser
                        TraversalCounters* counters, uint2* __restrict__ stack, WarpScratch& ws, uint& head, uint& tail)
     {
         const uint lane = threadIdx.x & 31u;
-        const uint octinv4 = octinv * 0x01010101u;
-        const bool negx = !(octinv & 4u), negy = !(octinv & 2u), negz = !(octinv & 1u);
         uint one; asm volatile("mov.b32 %0, 0x3F800000;" : "=r"(one));        // see byteToUnitFloatImm
         while (true)
         {
@@ -281,52 +388,9 @@ struct Traverser
                 }
                 if (COUNT) counters->nodeVisits++;
 
-                const float px = __uint_as_float(n0.x), py = __uint_as_float(n0.y), pz = __uint_as_float(n0.z);
-                // quantisation scale 2^(e-127) per axis, times 2^15 (bvh_builder.cpp keeps e + 15 < 255)
-                const float sx15 = __uint_as_float(((n0.w & 0xFFu) + 15u) << 23), sy15 = __uint_as_float((((n0.w >> 8) & 0xFFu) + 15u) << 23), sz15 = __uint_as_float((((n0.w >> 16) & 0xFFu) + 15u) << 23);
                 const uint imask = n0.w >> 24;
                 nodeGroup.x = n1.x; triBase = n1.y;
-                // Slab test on the quantised child boxes.  A quantised coordinate byte b is turned into the float m = 1 + b * 2^-15 with one
-                // byte permute (ALU pipe) instead of an integer->float conversion (quarter-rate XU pipe, the top pipe of this kernel in the
-                // round-1 ncu capture); then b * (s * id) + o == m * A + (o - A) with A = s * id * 2^15.  The box test only has to be
-                // conservative (the triangle test decides): the relative slack eps and an absolute pad that covers the rounding of (o - A)
-                // (<= 2^-22 (|A| + |o|), |o| <= |t| + 2^8 |s id|) are folded into the per-node constants, near planes pulled in, far pushed out.
-                // PT_I2F_AXES of the three axes keep the integer->float conversion (XU pipe) so that the conversions are spread over two pipes:
-                // for those, b * (s id) + o is evaluated directly (A = s id, no offset), with the same slack.
-                const float Ax15 = sx15 * idx, Ay15 = sy15 * idy, Az15 = sz15 * idz;
-                const float Ax = (PT_I2F_AXES > 0) ? Ax15 * (1.0f / 32768.0f) : Ax15, Ay = (PT_I2F_AXES > 1) ? Ay15 * (1.0f / 32768.0f) : Ay15, Az = (PT_I2F_AXES > 2) ? Az15 * (1.0f / 32768.0f) : Az15;
-                const float ox = (px - org.x) * idx, oy = (py - org.y) * idy, oz = (pz - org.z) * idz;
-                const float Ox = (PT_I2F_AXES > 0) ? ox : ox - Ax, Oy = (PT_I2F_AXES > 1) ? oy : oy - Ay, Oz = (PT_I2F_AXES > 2) ? oz : oz - Az;
-                const float kLo = 1.0f - 6.0e-7f, kHi = 1.0f + 6.0e-7f, kPad = 4.8e-7f;
-                const float Anx = Ax * kLo, Any = Ay * kLo, Anz = Az * kLo, Afx = Ax * kHi, Afy = Ay * kHi, Afz = Az * kHi;
-                const float Onx = __fmaf_rn(Ox, kLo, -fabsf(Ax15) * kPad), Ony = __fmaf_rn(Oy, kLo, -fabsf(Ay15) * kPad), Onz = __fmaf_rn(Oz, kLo, -fabsf(Az15) * kPad);
-                const float Ofx = __fmaf_rn(Ox, kHi, fabsf(Ax15) * kPad), Ofy = __fmaf_rn(Oy, kHi, fabsf(Ay15) * kPad), Ofz = __fmaf_rn(Oz, kHi, fabsf(Az15) * kPad);
-                uint hitmask = 0;
-                #pragma unroll
-                for (int half = 0; half < 2; half++)
-                {
-                    const uint meta4 = half ? n1.w : n1.z;
-                    const uint isInner4 = (meta4 & (meta4 << 1)) & 0x10101010u;
-                    const uint innerMask4 = (isInner4 >> 4) * 0xFFu;
-                    const uint bitIndex4 = (meta4 ^ (octinv4 & innerMask4)) & 0x1F1F1F1Fu;
-                    const uint childBits4 = (meta4 >> 5) & 0x07070707u;
-                    const uint qlox = half ? n2.y : n2.x, qloy = half ? n2.w : n2.z, qloz = half ? n3.y : n3.x;
-                    const uint qhix = half ? n3.w : n3.z, qhiy = half ? n4.y : n4.x, qhiz = half ? n4.w : n4.z;
-                    const uint nearx = negx ? qhix : qlox, farx = negx ? qlox : qhix;
-                    const uint neary = negy ? qhiy : qloy, fary = negy ? qloy : qhiy;
-                    const uint nearz = negz ? qhiz : qloz, farz = negz ? qloz : qhiz;
-                    #pragma unroll
-                    for (int j = 0; j < 4; j++)
-                    {
-                        const float t0x = __fmaf_rn(byteToCoord<(PT_I2F_AXES > 0)>(nearx, j, one), Anx, Onx), t1x = __fmaf_rn(byteToCoord<(PT_I2F_AXES > 0)>(farx, j, one), Afx, Ofx);
-                        const float t0y = __fmaf_rn(byteToCoord<(PT_I2F_AXES > 1)>(neary, j, one), Any, Ony), t1y = __fmaf_rn(byteToCoord<(PT_I2F_AXES > 1)>(fary, j, one), Afy, Ofy);
-                        const float t0z = __fmaf_rn(byteToCoord<(PT_I2F_AXES > 2)>(nearz, j, one), Anz, Onz), t1z = __fmaf_rn(byteToCoord<(PT_I2F_AXES > 2)>(farz, j, one), Afz, Ofz);
-                        const float cmin = fmaxf(fmaxf(t0x, t0y), fmaxf(t0z, tMin));
-                        const float cmax = fminf(fminf(t1x, t1y), fminf(t1z, bestT));
-                        if (cmin <= cmax)
-                            hitmask |= ((childBits4 >> (8 * j)) & 0xFFu) << ((bitIndex4 >> (8 * j)) & 0xFFu);
-                    }
-                }
+                const uint hitmask = nodeHitMask<TMIN_ZERO>(n0, n1, n2, n3, n4, org, idx, idy, idz, octinv, tMin, bestT, one);
                 nodeGroup.y = (hitmask & 0xFF000000u) | imask;
                 triBits = hitmask & 0x00FFFFFFu;
                 if (PT_PREFETCH_CHILDREN)
