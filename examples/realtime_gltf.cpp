@@ -1,7 +1,8 @@
 // realtime_gltf.cpp - the realtime side of the C ABI in one C++ host: load a glTF / .scene.json, then per frame what Sample::Render does around the realtime path tracer
 // (Rtxpt/Sample.cpp:1412, :2438-2618, ToneMappingPasses.cpp:230-360): LightsBaker feedback update -> stable-plane BUILD + FILL -> guide filter + per-plane ReBLUR + final merge ->
 // tone mapping; the last frame's SRGBA8 image is written as a PPM.  Static camera and scene (animation: rtxpt_b200_update_instance_transforms / rtxpt_b200_skin_update before the trace).
-//   realtime_gltf scene.gltf out.ppm [width height frames bounces]
+//   realtime_gltf scene.gltf out.ppm [width height frames bounces] [--approximate-mis]
+// --approximate-mis: approximate light-vs-BSDF MIS, what RTXPT's realtime mode compiles by default (SampleUI NEEMISType 1: ActualUseApproximateMIS() is true in realtime mode)
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -13,7 +14,10 @@ static int fail(const char* what, rtxpt_ctx* ctx) { fprintf(stderr, "%s: %s\n", 
 
 int main(int argc, char** argv)
 {
-    if (argc < 3) { fprintf(stderr, "usage: %s scene.gltf out.ppm [width height frames bounces]\n", argv[0]); return 2; }
+    bool approximateMIS = false;
+    for (int i = 1; i < argc; i++)
+        if (!strcmp(argv[i], "--approximate-mis")) { approximateMIS = true; for (int j = i; j + 1 < argc; j++) argv[j] = argv[j + 1]; argc--; i--; }
+    if (argc < 3) { fprintf(stderr, "usage: %s scene.gltf out.ppm [width height frames bounces] [--approximate-mis]\n", argv[0]); return 2; }
     const uint32_t width = argc > 3 ? uint32_t(atoi(argv[3])) : 512, height = argc > 4 ? uint32_t(atoi(argv[4])) : 512;
     const uint32_t frames = argc > 5 ? uint32_t(atoi(argv[5])) : 16, bounces = argc > 6 ? uint32_t(atoi(argv[6])) : 6;
     rtxpt_host_scene* scene = nullptr; uint32_t overridden = 0;
@@ -30,6 +34,7 @@ int main(int argc, char** argv)
     RtxptPathTracerConstants consts; rtxpt_b200_default_constants(&cam, 0, &consts);
     consts.bounceCount = bounces; consts.diffuseBounceCount = bounces < 3 ? bounces : 3;
     consts.NEEType = 2; consts.NEEATFeedback = 1; consts.NEEATImportanceBoost = 3;                     // RTXPT's defaults: NEE-AT with temporal feedback and both importance boosters
+    consts.useApproximateMIS = approximateMIS ? 1u : 0u;                                              // pt.useApproximateMIS = m_ui.ActualUseApproximateMIS()
     RtxptRealtimeConstants rt = {};
     rt.activeStablePlaneCount = 3; rt.maxStablePlaneVertexDepth = bounces < 14 ? bounces : 14; rt.allowPrimarySurfaceReplacement = 1; rt.subSampleCount = 1;
     memcpy(rt.matWorldToClipNoOffset, worldToClip, 64); memcpy(rt.prevMatWorldToClipNoOffset, worldToClip, 64);

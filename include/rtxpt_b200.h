@@ -250,7 +250,11 @@ typedef struct RtxptPathTracerConstants {
                                              * NEE, usage-weighted global table and per-tile local samplers, advanced once per frame by rtxpt_b200_neeat_update_begin / _end (SURVEY §8f row 1) */
     uint32_t NEEATImportanceBoost;          /* with NEEATFeedback: LightsBaker's importance boosters (LightsBaker.h:245-249, both on in RTXPT's UI): bit 0 lights in / near the view frustum (needs
                                              * rtxpt_b200_set_view), bit 1 lights that got brighter since the last frame; 0 = neither */
-    float    _pad[1];
+    uint32_t useApproximateMIS;             /* the resolved RTXPT_USE_APPROXIMATE_MIS macro (Sample.cpp:1015): 0 = full light-vs-BSDF MIS, 1 = approximate MIS, in which the light's
+                                             * selection x solid-angle pdf is replaced by the constant 3 on both sides and the BSDF side reads no light record (LightSampler.hlsli:271-280).
+                                             * RTXPT resolves it as SampleUI::ActualUseApproximateMIS() = RealtimeMode ? NEEMISType != 0 : NEEMISType == 2 (SampleUI.h:135), and its
+                                             * default NEEMISType 1 makes realtime mode approximate: pt.useApproximateMIS = m_ui.ActualUseApproximateMIS().  Values above 1 are refused
+                                             * (RTXPT_ERR_INVALID_ARGUMENT).  rtxpt_b200_default_constants gives 0. */
 } RtxptPathTracerConstants;
 
 /* ------------------------------------------------------------------------------------------------------------------

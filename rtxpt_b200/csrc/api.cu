@@ -622,6 +622,7 @@ extern "C" RTXPT_API int rtxpt_b200_set_constants(rtxpt_ctx* c, const RtxptPathT
 {
     if (!c || !k) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
     cudaSetDevice(c->device);
+    if (k->useApproximateMIS > 1) return fail(RTXPT_ERR_INVALID_ARGUMENT, "useApproximateMIS %u: 0 (full MIS) or 1 (approximate MIS)", k->useApproximateMIS);
     if (k->NEEFullSamples > 1 && k->NEEType == 2 && k->NEEATFeedback != 0)
         return fail(RTXPT_ERR_UNSUPPORTED, "NEEFullSamples > 1 together with NEE-AT temporal feedback is not supported: a visible sample's feedback draw decides the next sample's candidates, "
                                            "and the wavefront learns visibility only after the shadow kernel");

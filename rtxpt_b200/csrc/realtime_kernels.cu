@@ -123,8 +123,8 @@ __global__ void __launch_bounds__(256) k_rt_fill_generate(const __grid_constant_
                                 // H100 SXM (700 W): config-3 trace 41.5 ms/frame with 4, 42.4 with 3; the 1-spp realtime frame 9.69 ms with 4, 9.60 with 3
 #endif
 // MULTI (FILL pass, NEEFullSamples > 1): shadeHit appends the vertex's shadow records and NEE block itself, one record per valid light sample; 3 CTAs per SM, which
-// lets it run without spills in both builds
-template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false>
+// lets it run without spills in both builds.  AMIS (FILL pass): approximate light-vs-BSDF MIS; the BUILD pass evaluates no MIS (PathState.hlsli:157-159) and has one kernel for both kinds
+template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false>
 __global__ void __launch_bounds__(128, MULTI ? 3 : PT_RT_SHADE_CTAS) k_rt_shade(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
@@ -146,8 +146,8 @@ __global__ void __launch_bounds__(128, MULTI ? 3 : PT_RT_SHADE_CTAS) k_rt_shade(
                 const uint slot = queue[i];
                 PathRegs path; path.load(p.wf, slot, true);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
-                if (cls == 0) shadeMiss<false, MODE, NEEAT>(p, path);
-                else shadeHit<false, ANALYTIC_LIGHTS, MODE, NEEAT, MULTI>(p, path, slot, p.wf.hits[slot], out);
+                if (cls == 0) shadeMiss<false, MODE, NEEAT, AMIS>(p, path);
+                else shadeHit<false, ANALYTIC_LIGHTS, MODE, NEEAT, MULTI, AMIS>(p, path, slot, p.wf.hits[slot], out);
                 continues = (cls != 0) && out.continuePath;
                 if constexpr (MODE == kModeBuildStablePlanes)
                 {   // postProcessHit: when this branch has ended, continue with the next enqueued branch of the pixel (planes above the current one)
@@ -259,17 +259,29 @@ void launchDnFinalMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t
 
 void launchRtBuildGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_build_generate<<<g.smCount * 4, 256, 0, s>>>(p); }
 void launchRtFillGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_fill_generate<<<g.smCount * 4, 256, 0, s>>>(p); }
+template <bool AMIS>
+static void launchRtShadeNeeatMis(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
+{
+    const int grid = g.smCount * PT_RT_SHADE_CTAS;
+    if (p.scene.analyticLightCount != 0) k_rt_shade<kModeFillStablePlanes, true, true, false, AMIS><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeFillStablePlanes, false, true, false, AMIS><<<grid, 128, 0, s>>>(p);
+}
 void launchRtShadeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
 {   // FILL pass with NEE-AT feedback: tile-sampler candidates, MIS against the global table, feedback records for the shadow kernel
+    if (p.c.useApproximateMIS) launchRtShadeNeeatMis<true>(p, g, s); else launchRtShadeNeeatMis<false>(p, g, s);
+}
+template <bool AMIS>
+static void launchRtShadeFill(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
+{
     const int grid = g.smCount * PT_RT_SHADE_CTAS;
-    if (p.scene.analyticLightCount != 0) k_rt_shade<kModeFillStablePlanes, true, true><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeFillStablePlanes, false, true><<<grid, 128, 0, s>>>(p);
+    if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1) k_rt_shade<kModeFillStablePlanes, true, false, true, AMIS><<<g.smCount * 3, 128, 0, s>>>(p);      // several light samples per vertex: analytic lights gated at run time
+    else { if (p.scene.analyticLightCount != 0) k_rt_shade<kModeFillStablePlanes, true, false, false, AMIS><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeFillStablePlanes, false, false, false, AMIS><<<grid, 128, 0, s>>>(p); }
 }
 void launchRtShade(const LaunchParams& p, const GridConfig& g, bool fill, cudaStream_t s)
 {
     const int grid = g.smCount * PT_RT_SHADE_CTAS;
     if (!fill) { if (p.scene.analyticLightCount != 0) k_rt_shade<kModeBuildStablePlanes, true><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeBuildStablePlanes, false><<<grid, 128, 0, s>>>(p); }
-    else if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1) k_rt_shade<kModeFillStablePlanes, true, false, true><<<g.smCount * 3, 128, 0, s>>>(p);      // several light samples per vertex: analytic lights gated at run time
-    else { if (p.scene.analyticLightCount != 0) k_rt_shade<kModeFillStablePlanes, true><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeFillStablePlanes, false><<<grid, 128, 0, s>>>(p); }
+    else if (p.c.useApproximateMIS) launchRtShadeFill<true>(p, g, s);
+    else launchRtShadeFill<false>(p, g, s);
 }
 void launchRtFillCommit(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_fill_commit<<<g.smCount * 4, 256, 0, s>>>(p); }
 void launchRtMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_merge<<<g.smCount * 4, 256, 0, s>>>(p); }

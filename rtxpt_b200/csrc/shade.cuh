@@ -13,6 +13,8 @@
 // shadow kernel adds it to L — same arithmetic and order as ProcessLightSample followed by AccumulatePathRadiance.  With NEEFullSamples > 1
 // (MULTI) every valid light sample gets its own shadow record and parks its fp32 result in the vertex's NEE block (wavefront.cuh); the shadow
 // kernel marks the visible ones and k_nee_resolve sums them in sample order before the one AccumulatePathRadiance.
+// Light-vs-BSDF MIS comes in RTXPT's two kinds (RTXPT_USE_APPROXIMATE_MIS): full (ComputeLightVsBSDF_MIS_ForLight / ForBSDF, LightSampler.hlsli:282-331) and, with AMIS,
+// approximate (the _Approx pair, :271-280), a compile-time choice as in the reference; RtxptPathTracerConstants::useApproximateMIS selects the kernel.
 #pragma once
 #include "wavefront.cuh"
 #include "bsdf.cuh"
@@ -151,6 +153,12 @@ PT_DEVICE float misForBsdfT(const LaunchParams& p, uint pathId, uint misPacked, 
         return misBalance(bsdfPdf, lightAvgPdf * solidAnglePdf);
     }
 }
+// Approximate MIS (RTXPT_USE_APPROXIMATE_MIS = 1, LightSampler.hlsli:271-280): the light's selection x solid-angle pdf is replaced by the constant
+// RTXPT_NEEAT_MIS_APPROXIMATION_LIGHTSAMPLER_BIAS = 3 on both sides, so the BSDF side needs neither the light's index nor its record nor a sampler pdf.
+// EvalMIS(Balance, fullSamples * candidates, 3, 1, bsdfPdf) on the light side, EvalMIS(Balance, 1, bsdfPdf, fullSamples * candidates, 3) on the BSDF side.
+constexpr float kApproxMisLightSamplerBias = 3.0f;
+PT_DEVICE float misApproxForLight(uint fullSamples, uint candidateCount, float bsdfPdf) { return misBalance(float(fullSamples * candidateCount) * kApproxMisLightSamplerBias, bsdfPdf); }
+PT_DEVICE float misApproxForBsdf(uint misPacked, float bsdfPdf) { return misBalance(bsdfPdf, float((misPacked & 0x3F) * ((misPacked >> 6) & 0x3F)) * kApproxMisLightSamplerBias); }
 
 // ---- firefly filter (PathTracerHelpers.hlsli:183-219) ----------------------------------------------------------------------------
 PT_DEVICE float coneSpreadFromPdf(float pdf, float growth) { return growth * 2.0f * fastACos(fmaxf(-1.0f, 1.0f - (1.0f / pdf) / (2.0f * kPi))); }
@@ -223,7 +231,8 @@ PT_DEVICE float triangleCurvatureGradN(const float* xf, float3 p0, float3 p1, fl
 
 // MODE: the realtime passes also need the motion-vector controls of the surface (block heuristics: every realtime pass; last frame's position: BUILD pass only); the reference-mode
 // instantiation carries none of that code.  pathId = packed pixel, vertexIndex / sampleIndex seed the heuristic's MicroRng (BridgeDonut:714).
-template <int MODE>
+// AMIS (approximate MIS): the emissive triangle's light index is not looked up - nothing reads it (BridgeDonut:806-810).
+template <int MODE, bool AMIS = false>
 PT_DEVICE void loadSurface(const LaunchParams& p, uint gid, float bu, float bv, float3 rayDir, float coneWidth, Surface& s, uint pathId = 0, uint vertexIndex = 1, uint sampleIndex = 0)
 {
     const SceneView& sc = p.scene;
@@ -407,8 +416,11 @@ PT_DEVICE void loadSurface(const LaunchParams& p, uint gid, float bu, float bv, 
     if (frontFacing && anyPositive(emissiveColor))
     {
         s.emission = emissiveColor;
-        const uint baseIndex = sc.subInstances[subIndex].EmissiveLightMappingOffset;
-        if (baseIndex != 0xFFFFFFFFu) s.neeTriangleLightIndex = baseIndex + info.z;
+        if constexpr (!AMIS)
+        {
+            const uint baseIndex = sc.subInstances[subIndex].EmissiveLightMappingOffset;
+            if (baseIndex != 0xFFFFFFFFu) s.neeTriangleLightIndex = baseIndex + info.z;
+        }
     }
     s.interiorIoR = matIoR;
 }
@@ -454,7 +466,8 @@ PT_DEVICE void accumulatePathRadiance(const LaunchParams& p, PathRegs& path, flo
     }
 }
 
-template <bool EXPORT_GUIDES, int MODE = kModeReference, bool NEEAT = false>
+// AMIS: approximate light-vs-BSDF MIS (RTXPT_USE_APPROXIMATE_MIS = 1) at the environment miss, the emissive triangle, the analytic proxy and the light sample
+template <bool EXPORT_GUIDES, int MODE = kModeReference, bool NEEAT = false, bool AMIS = false>
 PT_DEVICE void shadeMiss(const LaunchParams& p, PathRegs& path)
 {
     const float3 segmentOrigin = path.origin;
@@ -469,7 +482,8 @@ PT_DEVICE void shadeMiss(const LaunchParams& p, PathRegs& path)
         const float3 Le = envEvalLocal(p, localDir, mip);
         float misWeight = 1.0f;
         const float bsdfPdf = (MODE == kModeBuildStablePlanes) ? 0.0f : path.bsdfScatterPdf();
-        if ((mis & (1u << 15)) && bsdfPdf != 0)
+        if constexpr (AMIS) { if ((mis & (1u << 15)) && bsdfPdf != 0) misWeight = misApproxForBsdf(mis, bsdfPdf); }         // PathTracer.hlsli:461-462: no quad-tree lookup
+        else if ((mis & (1u << 15)) && bsdfPdf != 0)
         {
             const float2 uv = dirToOctEqualArea(localDir);
             const uint cx = min(uint(uv.x * float(kEnvLookupDim)), kEnvLookupDim - 1), cy = min(uint(uv.y * float(kEnvLookupDim)), kEnvLookupDim - 1);
@@ -506,7 +520,7 @@ PT_DEVICE void addFillSpecAvgChoice(uint& word, uint preFlags, uint preCounters)
 
 // MULTI: NEEFullSamples > 1 - the light samples' shadow records and the vertex's NEE block go straight to the launch's arrays (out.emitShadow stays false).  Without
 // NEE-AT feedback no draw depends on visibility, so the samples are drawn one after the other from the vertex's one uniform stream as HandleNEE draws them.
-template <bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, int MODE = kModeReference, bool NEEAT = false, bool MULTI = false>
+template <bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, int MODE = kModeReference, bool NEEAT = false, bool MULTI = false, bool AMIS = false>
 PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4 hit, HitOutputs& out)
 {
     out.continuePath = false; out.emitShadow = false;
@@ -531,7 +545,7 @@ PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4
 #ifdef PT_HOST_EMU
     emuLoadSurface(s);
 #else
-    loadSurface<MODE>(p, __float_as_uint(hit.w), hit.y, hit.z, rayDir, path.coneWidth(), s, path.id, path.vertexIndex(), sampleIndex);
+    loadSurface<MODE, AMIS>(p, __float_as_uint(hit.w), hit.y, hit.z, rayDir, path.coneWidth(), s, path.id, path.vertexIndex(), sampleIndex);
 #endif
     const uint ndq = p.c.nestedDielectricsQuality;
     if (ndq > 0 && path.interior0 != 0)
@@ -575,7 +589,9 @@ PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4
     {
         float misWeight = 1.0f;
         const float bsdfPdf = pathBsdfPdf;
-        if ((misPacked & (1u << 15)) && bsdfPdf != 0 && s.neeTriangleLightIndex != kInvalidLight)
+        // approximate MIS weights every emitter on the BSDF side, one without a light record too (ExcludeFromNEE, light-list overflow): PathTracer.hlsli:619-620 tests no index
+        if constexpr (AMIS) { if ((misPacked & (1u << 15)) && bsdfPdf != 0) misWeight = misApproxForBsdf(misPacked, bsdfPdf); }
+        else if ((misPacked & (1u << 15)) && bsdfPdf != 0 && s.neeTriangleLightIndex != kInvalidLight)
         {
             TriLight tl; tl.decode(p.scene.lights[s.neeTriangleLightIndex]);
             misWeight = misForBsdfT<NEEAT>(p, path.id, misPacked, s.neeTriangleLightIndex, bsdfPdf, tl.solidAnglePdfForMIS(rayOrigin, s.posW));
@@ -599,7 +615,8 @@ PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4
                     const float3 radiance = unpackLightRadiance(li) * lightShaping(li, p.scene, s.neeAnalyticLightIndex, rayOrigin, center);
                     float mis = 1.0f;
                     const float bsdfPdf = (misPacked & (1u << 15)) ? pathBsdfPdf : 0.0f;
-                    if (bsdfPdf != 0)
+                    if (AMIS && bsdfPdf != 0) mis = misApproxForBsdf(misPacked, bsdfPdf);
+                    else if (bsdfPdf != 0)
                     {
                         const float cosThetaMax = sqrtf(fmaxf(0.0f, 1.0f - (radius * radius) / dot3(lv, lv)));
                         mis = misForBsdfT<NEEAT>(p, path.id, misPacked, s.neeAnalyticLightIndex, bsdfPdf, 1.0f / (2.0f * kPi * (1.0f - cosThetaMax)));
@@ -827,7 +844,8 @@ PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4
                 }
                 const float wrsMIS = misBalance(pickSelPdf, otherPdf) / thisCount;             // without feedback all candidates come from the global table
                 const float scatterPdfForDir = bsdf.pdf(pickDir);
-                const float pathMIS = misBalance((pickSelPdf + otherPdf) * float(fullSamples) * pickSolidPdf, pickBsdfSampleable ? scatterPdfForDir : 0.0f);    // LightSampleableByBSDF
+                const float pathMIS = AMIS ? misApproxForLight(fullSamples, candidateCount, pickBsdfSampleable ? scatterPdfForDir : 0.0f)     // PathTracerNEE.hlsli:228-229
+                                           : misBalance((pickSelPdf + otherPdf) * float(fullSamples) * pickSolidPdf, pickBsdfSampleable ? scatterPdfForDir : 0.0f);    // LightSampleableByBSDF
                 const float3 Li = pickLi * (fadeOut * wrsMIS * pathMIS / float(fullSamples));
                 const float4 bsdfThp = bsdf.eval(pickDir);
                 float3 radiance = mk3(bsdfThp.x, bsdfThp.y, bsdfThp.z) * Li;

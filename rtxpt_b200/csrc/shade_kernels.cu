@@ -39,7 +39,8 @@ void launchInitTables(cudaStream_t s) { k_init_sobol_tables<<<16, 256, 0, s>>>()
 
 // ---- shade --------------------------------------------------------------------------------------------------------------------------------
 // MULTI (NEEFullSamples > 1): shadeHit appends the vertex's shadow records and NEE block itself, one record per valid light sample
-template <int MINB, bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false>
+// AMIS: approximate light-vs-BSDF MIS (RtxptPathTracerConstants::useApproximateMIS = 1); a template argument, as RTXPT compiles it in
+template <int MINB, bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false>
 __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
@@ -61,8 +62,8 @@ __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ Lau
                 const uint r = queue[i];
                 h = path.loadRay(p.stateIn, r, p.radiance);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
-                if (cls == 0) shadeMiss<EXPORT_GUIDES, kModeReference, NEEAT>(p, path);
-                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT, MULTI>(p, path, h, p.wf.hits[r], out);
+                if (cls == 0) shadeMiss<EXPORT_GUIDES, kModeReference, NEEAT, AMIS>(p, path);
+                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT, MULTI, AMIS>(p, path, h, p.wf.hits[r], out);
                 path.storeRadiance(p.radiance, h);
                 if (out.continuePath) rayCls = 0;
                 if (out.emitShadow) shadowCls = 0;
@@ -111,22 +112,31 @@ __global__ void k_debug_rng(const uint* __restrict__ in, uint count, uint* __res
     for (uint k = 0; k < 4; k++) out[i * 8 + 4 + k] = __float_as_uint(hashToFloat(ldSampleBits(baseHash, in[i * 4 + 3], 1u, k)));
 }
 
-// reference mode with NEE-AT feedback: one instantiation (guides on: the feedback passes reproject with them; analytic lights compiled in, gated by the light type at run time)
-void launchShadeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_shade<3, true, true, true><<<g.smCount * 3, 128, 0, s>>>(p); }      // 3 CTAs per SM: 155 registers, no spills
-void launchShade(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
+// reference mode with NEE-AT feedback: one instantiation per MIS kind (guides on: the feedback passes reproject with them; analytic lights compiled in, gated by the light type at run time)
+void launchShadeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s)       // 3 CTAs per SM: 155 registers, no spills
+{
+    if (p.c.useApproximateMIS) k_shade<3, true, true, true, false, true><<<g.smCount * 3, 128, 0, s>>>(p); else k_shade<3, true, true, true><<<g.smCount * 3, 128, 0, s>>>(p);
+}
+// the same choice of kernel for either MIS kind: the approximate kernels are the full-MIS ones with AMIS set
+template <bool AMIS>
+static void launchShadeMis(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
 {
     const int grid = g.smCount * g.shadeBlocksPerSM;
     // guide export and analytic (sphere) lights are separate instantiations: the default kernel carries neither
     if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1)
     {   // several light samples per vertex: analytic lights compiled in, gated by the light type at run time
-        if (p.exportGuides) k_shade<3, true, true, false, true><<<g.smCount * 3, 128, 0, s>>>(p); else k_shade<3, false, true, false, true><<<g.smCount * 3, 128, 0, s>>>(p);
+        if (p.exportGuides) k_shade<3, true, true, false, true, AMIS><<<g.smCount * 3, 128, 0, s>>>(p); else k_shade<3, false, true, false, true, AMIS><<<g.smCount * 3, 128, 0, s>>>(p);
         return;
     }
-    if (p.exportGuides) { k_shade<4, true, true><<<g.smCount * 4, 128, 0, s>>>(p); return; }
-    if (p.scene.analyticLightCount != 0) { k_shade<4, false, true><<<g.smCount * 4, 128, 0, s>>>(p); return; }
-    if (g.shadeBlocksPerSM >= 5) k_shade<5, false, false><<<grid, 128, 0, s>>>(p);
-    else if (g.shadeBlocksPerSM == 4) k_shade<4, false, false><<<grid, 128, 0, s>>>(p);
-    else k_shade<3, false, false><<<grid, 128, 0, s>>>(p);
+    if (p.exportGuides) { k_shade<4, true, true, false, false, AMIS><<<g.smCount * 4, 128, 0, s>>>(p); return; }
+    if (p.scene.analyticLightCount != 0) { k_shade<4, false, true, false, false, AMIS><<<g.smCount * 4, 128, 0, s>>>(p); return; }
+    if (g.shadeBlocksPerSM >= 5) k_shade<5, false, false, false, false, AMIS><<<grid, 128, 0, s>>>(p);
+    else if (g.shadeBlocksPerSM == 4) k_shade<4, false, false, false, false, AMIS><<<grid, 128, 0, s>>>(p);
+    else k_shade<3, false, false, false, false, AMIS><<<grid, 128, 0, s>>>(p);
+}
+void launchShade(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
+{
+    if (p.c.useApproximateMIS) launchShadeMis<true>(p, g, s); else launchShadeMis<false>(p, g, s);
 }
 void launchDebugBsdf(const float* in, uint32_t count, float* out, cudaStream_t s) { k_debug_bsdf<<<(count + 127) / 128, 128, 0, s>>>(in, count, out); }
 void launchDebugRng(const uint32_t* in, uint32_t count, uint32_t* out, cudaStream_t s) { k_debug_rng<<<(count + 127) / 128, 128, 0, s>>>(in, count, out); }

@@ -431,7 +431,7 @@ def bridge_camera(width, height, pos, direction, up, fov_y, near_z=0.1, far_z=1e
 
 def make_constants(width, height, camera, bounce_count=6, diffuse_bounce_count=6, sample_base_index=0, nee=True, nee_type=2,
                    firefly_threshold=0.0, env_enabled=False, env_color=(1, 1, 1), russian_roulette=True, ld_sampler=True, nested_dielectrics=1,
-                   aa_jitter=1.0, tex_lod_bias=-1.0, nee_candidates=5, nee_full=1, env_mip=2.0, distant_vs_local=1.0):
+                   aa_jitter=1.0, tex_lod_bias=-1.0, nee_candidates=5, nee_full=1, env_mip=2.0, distant_vs_local=1.0, approximate_mis=False):
     c = S.PathTracerConstants()
     c.imageWidth, c.imageHeight, c.sampleBaseIndex = width, height, sample_base_index
     c.perPixelJitterAAScale = aa_jitter
@@ -445,4 +445,5 @@ def make_constants(width, height, camera, bounce_count=6, diffuse_bounce_count=6
     c.envMap.Transform[:] = ident; c.envMap.InvTransform[:] = ident
     c.envMap.ColorMultiplier[:] = env_color; c.envMap.Enabled = 1.0 if env_enabled else 0.0
     c.distantVsLocalImportance = distant_vs_local
+    c.useApproximateMIS = int(approximate_mis)
     return c

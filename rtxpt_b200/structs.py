@@ -195,7 +195,7 @@ class PathTracerConstants(C.Structure):
                 ("fireflyFilterThreshold", f32), ("NEEEnabled", u32), ("NEEType", u32), ("NEECandidateSamples", u32),
                 ("NEEFullSamples", u32), ("enableRussianRoulette", u32), ("enableLDSamplerForBSDF", u32),
                 ("nestedDielectricsQuality", u32), ("camera", CameraData), ("envMap", EnvMapSceneParams),
-                ("distantVsLocalImportance", f32), ("NEEATFeedback", u32), ("NEEATImportanceBoost", u32), ("_pad", f32 * 1)]
+                ("distantVsLocalImportance", f32), ("NEEATFeedback", u32), ("NEEATImportanceBoost", u32), ("useApproximateMIS", u32)]
 
 
 class Config(C.Structure):
