@@ -293,6 +293,29 @@ RTXPT_API int rtxpt_b200_upload_scene(rtxpt_ctx* ctx, const RtxptSceneDesc* scen
  * environment parameters changed. */
 RTXPT_API int rtxpt_b200_set_constants(rtxpt_ctx* ctx, const RtxptPathTracerConstants* constants);
 
+/* Stochastic texture filtering (RTXTF, External/Rtxtf; RTXPT_STOCHASTIC_TEXTURE_FILTERING_ENABLE = 1 in Rtxpt/Shaders/PathTracer/Config.h:95).  RTXPT passes STFFilterMode,
+ * STFMagnificationMethod and STFGaussianSigma (Sample.cpp:1466-1495, :1549-1555).  With `enable` set, every material texture fetch of every path-tracer pass (reference, BUILD,
+ * FILL) goes through STF_SamplerState::Texture2DSampleLevel at the ray-cone lambda: one stochastic integer mip and one stochastic texel of the filter at that mip, fetched at its
+ * centre, with the vertex's uniform numbers drawn as PathTracerBridgeDonut.hlsli:637-652 draws them.  Alpha testing, opacity masks, the environment and the emissive bake do not
+ * use the texture sampler in RTXPT either and are unaffected.  Off (the default) renders exactly as a context that never called this.
+ *   filterType:          STF_FILTER_TYPE_POINT 0, LINEAR 1, CUBIC 2, GAUSSIAN 3 (STFDefinitions.h); anything else is RTXPT_ERR_INVALID_ARGUMENT
+ *   magnificationMethod: STF_MAGNIFICATION_METHOD_NONE 0 only, RTXPT's default.  Methods 1-6 (2x2 quad / fine / fine temporal, 3x3 fine ALU / LUT, 4x4 fine) mix the texels of
+ *                        neighbouring lanes through WaveReadLaneAt (_Tex2D2x2WaveImpl, _Tex2D3x3WaveImpl, _Tex2D4x4WaveImpl): their result depends on which paths share a wave,
+ *                        which in a wavefront with class-sorted queues has no reproducible equivalent, so they are refused with RTXPT_ERR_UNSUPPORTED
+ *   gaussianSigma:       the Gaussian's standard deviation in texels (0.3 in RTXPT's UI); must be finite and positive (RTXPT_ERR_INVALID_ARGUMENT), read for every filter type
+ * A refused description leaves the context's setting as it was.  Applies from the next path_trace / path_trace_realtime. */
+typedef struct RtxptStochasticTextureFiltering {
+    uint32_t enable;
+    uint32_t filterType;
+    uint32_t magnificationMethod;
+    float    gaussianSigma;
+} RtxptStochasticTextureFiltering;
+#define RTXPT_STF_FILTER_TYPE_POINT     0u
+#define RTXPT_STF_FILTER_TYPE_LINEAR    1u
+#define RTXPT_STF_FILTER_TYPE_CUBIC     2u
+#define RTXPT_STF_FILTER_TYPE_GAUSSIAN  3u
+RTXPT_API int rtxpt_b200_set_texture_filtering(rtxpt_ctx* ctx, const RtxptStochasticTextureFiltering* stf);
+
 /* Replaces the loop body of Sample::PathTrace (Rtxpt/Sample.cpp:2503-2517): setPushConstants({subSampleIndex}) +
  * dispatchRays(width,height), for subSampleCount consecutive sub-samples starting at firstSubSampleIndex, each followed
  * by the reference-mode accumulation (AccumulationPass::Render, Rtxpt/Sample.cpp:2770-2778) when accumulate != 0.

@@ -83,7 +83,11 @@ using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
 using Event = Owned<cudaEvent_t, cudaEventDestroy>;
 
 // members are destroyed in reverse order: the texture object before its array
-struct DeviceTexture { Owned<cudaMipmappedArray_t, cudaFreeMipmappedArray> array; Owned<cudaTextureObject_t, cudaDestroyTextureObject> object; };
+struct DeviceTexture
+{
+    Owned<cudaMipmappedArray_t, cudaFreeMipmappedArray> array; Owned<cudaTextureObject_t, cudaDestroyTextureObject> object;
+    Owned<cudaTextureObject_t, cudaDestroyTextureObject> pointObject;         // the same arrays, point-filtered: stochastic texture filtering fetches one texel
+};
 
 struct rtxpt_ctx
 {
@@ -111,6 +115,8 @@ struct rtxpt_ctx
     DeviceArray<RtxptMaterialData> dMaterials; DeviceArray<uint8_t> dSubInstanceClass;
     std::vector<DeviceArray<uint8_t>> bufferAllocs; DeviceArray<const uint8_t*> dBufferTable;
     std::vector<DeviceTexture> textures; DeviceArray<cudaTextureObject_t> dTextureTable;
+    DeviceArray<cudaTextureObject_t> dPointTextureTable; DeviceArray<uint4> dTextureDims;     // stochastic texture filtering: point-filtered objects, width / height / levels
+    RtxptStochasticTextureFiltering stf{};                                                  // rtxpt_b200_set_texture_filtering (off)
     DeviceTexture envCube; uint32_t envFaceSize = 0, envMipLevels = 0;
     // rtxpt_b200_update_env_map: the bake's linear MIP chain and the importance map's, grown to the largest cube baked and never shrunk; the source of the last update, kept so
     // that the next update can re-bake from it; event times of the last update (bake, importance map, copy into the cube, readback + light bake + upload)
@@ -318,6 +324,8 @@ static int createTexture2D(const RtxptTextureDesc& d, DeviceTexture& out)
     // (measured with scripts/probes/bc_probe.cu: the *SRGB block-compressed kinds are refused without td.sRGB, every block-compressed kind is refused with cudaReadModeElementType)
     td.normalizedCoords = 1; td.maxAnisotropy = 1; td.minMipmapLevelClamp = 0; td.maxMipmapLevelClamp = float(d.mipLevels - 1);
     CU(out.object.create(cudaCreateTextureObject, &res, &td, nullptr));
+    td.filterMode = cudaFilterModePoint; td.mipmapFilterMode = cudaFilterModePoint;      // at a texel centre of an integer level: the texel itself, whatever the format
+    CU(out.pointObject.create(cudaCreateTextureObject, &res, &td, nullptr));
     return RTXPT_OK;
 }
 
@@ -504,8 +512,16 @@ extern "C" RTXPT_API int rtxpt_b200_upload_scene(rtxpt_ctx* c, const RtxptSceneD
     // bindless textures
     std::vector<cudaTextureObject_t> texTable(sc->textureCount, 0);
     c->textures.resize(sc->textureCount);
-    for (uint32_t i = 0; i < sc->textureCount; i++) { int rc = createTexture2D(sc->textures[i], c->textures[i]); if (rc != RTXPT_OK) return rc; texTable[i] = c->textures[i].object; }
+    std::vector<cudaTextureObject_t> pointTable(sc->textureCount, 0); std::vector<uint4> texDims(sc->textureCount);
+    for (uint32_t i = 0; i < sc->textureCount; i++)
+    {
+        int rc = createTexture2D(sc->textures[i], c->textures[i]); if (rc != RTXPT_OK) return rc;
+        texTable[i] = c->textures[i].object; pointTable[i] = c->textures[i].pointObject;
+        texDims[i] = make_uint4(sc->textures[i].width, sc->textures[i].height, sc->textures[i].mipLevels, 0u);
+    }
     CU(c->dTextureTable.upload(texTable.data(), texTable.size(), s));
+    CU(c->dPointTextureTable.upload(pointTable.data(), pointTable.size(), s));
+    CU(c->dTextureDims.upload(texDims.data(), texDims.size(), s));
     c->envFaceSize = sc->envCube.faceSize; c->envMipLevels = sc->envCube.mipLevels;
     if (sc->envCube.faceSize) { int rc = createEnvCube(sc->envCube, c->envCube); if (rc != RTXPT_OK) return rc; }
     // sub-instances: shade-queue class (the SER sort key analogue; the reference sorts by material permutation, MaterialsBaker.cpp:1227-1285)
@@ -636,6 +652,20 @@ extern "C" RTXPT_API int rtxpt_b200_set_constants(rtxpt_ctx* c, const RtxptPathT
     return RTXPT_OK;
 }
 
+extern "C" RTXPT_API int rtxpt_b200_set_texture_filtering(rtxpt_ctx* c, const RtxptStochasticTextureFiltering* f)
+{
+    if (!c || !f) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (f->enable > 1) return fail(RTXPT_ERR_INVALID_ARGUMENT, "enable %u: 0 or 1", f->enable);
+    if (f->filterType > RTXPT_STF_FILTER_TYPE_GAUSSIAN) return fail(RTXPT_ERR_INVALID_ARGUMENT, "filterType %u: STF_FILTER_TYPE_POINT (0) .. STF_FILTER_TYPE_GAUSSIAN (3)", f->filterType);
+    if (!(std::isfinite(f->gaussianSigma) && f->gaussianSigma > 0.0f)) return fail(RTXPT_ERR_INVALID_ARGUMENT, "gaussianSigma %g: finite and positive", double(f->gaussianSigma));
+    if (f->magnificationMethod > 6) return fail(RTXPT_ERR_INVALID_ARGUMENT, "magnificationMethod %u: STF_MAGNIFICATION_METHOD_NONE (0) .. 4x4_FINE (6)", f->magnificationMethod);
+    if (f->magnificationMethod != 0)
+        return fail(RTXPT_ERR_UNSUPPORTED, "magnificationMethod %u: the wave magnification methods mix texels of whichever lanes share a wave, which the wavefront's sorted queues "
+                                           "cannot reproduce; only STF_MAGNIFICATION_METHOD_NONE (0) is supported", f->magnificationMethod);
+    c->stf = *f;
+    return RTXPT_OK;
+}
+
 // ---- launch --------------------------------------------------------------------------------------------------------------------------------
 static void fillParams(rtxpt_ctx* c, LaunchParams& p)
 {
@@ -654,6 +684,10 @@ static void fillParams(rtxpt_ctx* c, LaunchParams& p)
     w.shadowOriginTMax = c->shadowOriginTMax.ptr; w.shadowDirPath = c->shadowDirPath.ptr; w.shadowRadiance = c->shadowRadiance.ptr;
     w.counters = c->counters.ptr; w.pixelOfSlot = c->pixelOfSlot.ptr; w.capacity = c->capacity; w.pixelCount = c->pixelCount;
     p.stateIn = StateSet{ c->s0.ptr, c->s1.ptr, c->s2.ptr, c->s3.ptr, c->s4.ptr }; p.stateOut = StateSet{ c->t0.ptr, c->t1.ptr, c->t2.ptr, c->t3.ptr, c->t4.ptr }; p.radiance = c->radiance.ptr;
+    if (c->stf.enable && c->dPointTextureTable.ptr)
+    {   // stochastic texture filtering: the launchers pick the STF kernels when the table is set
+        p.stf.pointTextures = c->dPointTextureTable.ptr; p.stf.textureDims = c->dTextureDims.ptr; p.stf.filterType = c->stf.filterType; p.stf.sigma = c->stf.gaussianSigma;
+    }
     p.c = c->consts;
     p.flags = c->cfg.flags;
     p.refillThreshold = c->tune.refillThreshold; p.waitFlushLanes = c->tune.waitFlushLanes;

@@ -124,8 +124,9 @@ __global__ void __launch_bounds__(256) k_rt_fill_generate(const __grid_constant_
 #endif
 // MULTI (FILL pass, NEEFullSamples > 1): shadeHit appends the vertex's shadow records and NEE block itself, one record per valid light sample; 3 CTAs per SM, which
 // lets it run without spills in both builds.  AMIS (FILL pass): approximate light-vs-BSDF MIS; the BUILD pass evaluates no MIS (PathState.hlsli:157-159) and has one kernel for both kinds
-template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false>
-__global__ void __launch_bounds__(128, MULTI ? 3 : PT_RT_SHADE_CTAS) k_rt_shade(const __grid_constant__ LaunchParams p)
+// STF: stochastic texture filtering of the material fetches (rtxpt_b200_set_texture_filtering); its kernels carry analytic lights, gated by the light type at run time
+template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false>
+__global__ void __launch_bounds__(128, (MULTI || STF) ? 3 : PT_RT_SHADE_CTAS) k_rt_shade(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
     uint* ctrNext = ctr + kCountersPerIter;
@@ -147,7 +148,7 @@ __global__ void __launch_bounds__(128, MULTI ? 3 : PT_RT_SHADE_CTAS) k_rt_shade(
                 PathRegs path; path.load(p.wf, slot, true);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
                 if (cls == 0) shadeMiss<false, MODE, NEEAT, AMIS>(p, path);
-                else shadeHit<false, ANALYTIC_LIGHTS, MODE, NEEAT, MULTI, AMIS>(p, path, slot, p.wf.hits[slot], out);
+                else shadeHit<false, ANALYTIC_LIGHTS, MODE, NEEAT, MULTI, AMIS, STF>(p, path, slot, p.wf.hits[slot], out);
                 continues = (cls != 0) && out.continuePath;
                 if constexpr (MODE == kModeBuildStablePlanes)
                 {   // postProcessHit: when this branch has ended, continue with the next enqueued branch of the pixel (planes above the current one)
@@ -263,6 +264,7 @@ template <bool AMIS>
 static void launchRtShadeNeeatMis(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
 {
     const int grid = g.smCount * PT_RT_SHADE_CTAS;
+    if (p.stf.pointTextures) { k_rt_shade<kModeFillStablePlanes, true, true, false, AMIS, true><<<g.smCount * 3, 128, 0, s>>>(p); return; }
     if (p.scene.analyticLightCount != 0) k_rt_shade<kModeFillStablePlanes, true, true, false, AMIS><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeFillStablePlanes, false, true, false, AMIS><<<grid, 128, 0, s>>>(p);
 }
 void launchRtShadeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
@@ -273,12 +275,19 @@ template <bool AMIS>
 static void launchRtShadeFill(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
 {
     const int grid = g.smCount * PT_RT_SHADE_CTAS;
+    if (p.stf.pointTextures)
+    {
+        if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1) k_rt_shade<kModeFillStablePlanes, true, false, true, AMIS, true><<<g.smCount * 3, 128, 0, s>>>(p);
+        else k_rt_shade<kModeFillStablePlanes, true, false, false, AMIS, true><<<g.smCount * 3, 128, 0, s>>>(p);
+        return;
+    }
     if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1) k_rt_shade<kModeFillStablePlanes, true, false, true, AMIS><<<g.smCount * 3, 128, 0, s>>>(p);      // several light samples per vertex: analytic lights gated at run time
     else { if (p.scene.analyticLightCount != 0) k_rt_shade<kModeFillStablePlanes, true, false, false, AMIS><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeFillStablePlanes, false, false, false, AMIS><<<grid, 128, 0, s>>>(p); }
 }
 void launchRtShade(const LaunchParams& p, const GridConfig& g, bool fill, cudaStream_t s)
 {
     const int grid = g.smCount * PT_RT_SHADE_CTAS;
+    if (!fill && p.stf.pointTextures) { k_rt_shade<kModeBuildStablePlanes, true, false, false, false, true><<<g.smCount * 3, 128, 0, s>>>(p); return; }
     if (!fill) { if (p.scene.analyticLightCount != 0) k_rt_shade<kModeBuildStablePlanes, true><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeBuildStablePlanes, false><<<grid, 128, 0, s>>>(p); }
     else if (p.c.useApproximateMIS) launchRtShadeFill<true>(p, g, s);
     else launchRtShadeFill<false>(p, g, s);

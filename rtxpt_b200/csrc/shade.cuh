@@ -18,6 +18,7 @@
 #pragma once
 #include "wavefront.cuh"
 #include "bsdf.cuh"
+#include "stf.cuh"
 
 namespace pt {
 
@@ -28,6 +29,18 @@ PT_DEVICE float4 sampleMaterialTexture(const SceneView& sc, uint textureIndexAnd
     float lambda = 0.5f * float(baseLOD) + lodNoDims;
     lambda = fminf(lambda, fmaxf(float(mipLevels) - 5.0f, 0.0f));
     return tex2DLod<float4>(sc.textures[textureIndex], uv.x, uv.y, lambda);
+}
+// Stochastic texture filtering (rtxpt_b200_set_texture_filtering): ExplicitRayConesLodTextureSampler's lambda, then STF_SamplerState::Texture2DSampleLevel - one texel of one integer
+// level, fetched at its centre through the point-filtered object over the same mip arrays, so that the texture unit returns the texel itself.  `stf` arrives by value: the bridge hands
+// the sampler to every fetch as a copy (sampleTexture's `const ActiveTextureSampler` parameter, BridgeDonut:269-278), so each fetch of a vertex starts from the vertex's state.
+PT_DEVICE float4 sampleMaterialTextureStf(const LaunchParams& p, uint textureIndexAndInfo, float lodNoDims, float2 uv, StfState stf)
+{
+    const uint textureIndex = textureIndexAndInfo & 0xFFFF, baseLOD = textureIndexAndInfo >> 24, mipLevels = (textureIndexAndInfo >> 16) & 0xFF;
+    float lambda = 0.5f * float(baseLOD) + lodNoDims;
+    lambda = fminf(lambda, fmaxf(float(mipLevels) - 5.0f, 0.0f));
+    const uint4 dims = p.stf.textureDims[textureIndex];             // Texture2D::GetDimensions(0, ...): width, height, number of levels
+    const StfSamplePos pos = stfTexture2DSamplePos(stf, dims.x, dims.y, dims.z, uv, lambda);
+    return tex2DLod<float4>(p.stf.pointTextures[textureIndex], pos.uv.x, pos.uv.y, float(pos.lod));
 }
 PT_DEVICE float safeLog2(float x) { return log2f(clampf(x, kFltMin, kFltMax)); }
 
@@ -232,7 +245,8 @@ PT_DEVICE float triangleCurvatureGradN(const float* xf, float3 p0, float3 p1, fl
 // MODE: the realtime passes also need the motion-vector controls of the surface (block heuristics: every realtime pass; last frame's position: BUILD pass only); the reference-mode
 // instantiation carries none of that code.  pathId = packed pixel, vertexIndex / sampleIndex seed the heuristic's MicroRng (BridgeDonut:714).
 // AMIS (approximate MIS): the emissive triangle's light index is not looked up - nothing reads it (BridgeDonut:806-810).
-template <int MODE, bool AMIS = false>
+// STF: the material textures are fetched through stochastic texture filtering (sampleMaterialTextureStf) with the vertex's sampler state (BridgeDonut:637-656).
+template <int MODE, bool AMIS = false, bool STF = false>
 PT_DEVICE void loadSurface(const LaunchParams& p, uint gid, float bu, float bv, float3 rayDir, float coneWidth, Surface& s, uint pathId = 0, uint vertexIndex = 1, uint sampleIndex = 0)
 {
     const SceneView& sc = p.scene;
@@ -310,12 +324,26 @@ PT_DEVICE void loadSurface(const LaunchParams& p, uint gid, float bu, float bv, 
 
     // sampleGeometryMaterialRTXPT + EvaluateSceneMaterialRTXPT
     float4 texBase = make_float4(1, 1, 1, 1), texMR = texBase, texEmissive = texBase, texNormal = make_float4(0.5f, 0.5f, 1.0f, 0.0f);
-    if (mflags & RTXPT_MATFLAG_UseBaseOrDiffuseTexture) texBase = sampleMaterialTexture(sc, m.BaseOrDiffuseTextureIndex, lodNoDims, uv);
-    if (mflags & RTXPT_MATFLAG_UseEmissiveTexture) texEmissive = sampleMaterialTexture(sc, m.EmissiveTextureIndex, lodNoDims, uv);
-    if (mflags & RTXPT_MATFLAG_UseNormalTexture) texNormal = sampleMaterialTexture(sc, m.NormalTextureIndex, lodNoDims, uv);
-    if (mflags & RTXPT_MATFLAG_UseMetalRoughOrSpecularTexture) texMR = sampleMaterialTexture(sc, m.MetalRoughOrSpecularTextureIndex, lodNoDims, uv);
     float texTrans = 1.0f;
-    if (mflags & RTXPT_MATFLAG_UseTransmissionTexture) texTrans = sampleMaterialTexture(sc, m.TransmissionTextureIndex, lodNoDims, uv).x;
+    if constexpr (STF)
+    {   // the bridge's five fetches in its order and under its conditions (BridgeDonut:402-423)
+        StfState stf;
+        stf.u = stfVertexRandom(pathId, vertexIndex, sampleIndex);
+        stf.filterType = p.stf.filterType; stf.sigma = p.stf.sigma; stf.reseedOnSample = false;
+        if (mflags & RTXPT_MATFLAG_UseBaseOrDiffuseTexture) texBase = sampleMaterialTextureStf(p, m.BaseOrDiffuseTextureIndex, lodNoDims, uv, stf);
+        if (mflags & RTXPT_MATFLAG_UseEmissiveTexture) texEmissive = sampleMaterialTextureStf(p, m.EmissiveTextureIndex, lodNoDims, uv, stf);
+        if (mflags & RTXPT_MATFLAG_UseNormalTexture) texNormal = sampleMaterialTextureStf(p, m.NormalTextureIndex, lodNoDims, uv, stf);
+        if (mflags & RTXPT_MATFLAG_UseMetalRoughOrSpecularTexture) texMR = sampleMaterialTextureStf(p, m.MetalRoughOrSpecularTextureIndex, lodNoDims, uv, stf);
+        if (mflags & RTXPT_MATFLAG_UseTransmissionTexture) texTrans = sampleMaterialTextureStf(p, m.TransmissionTextureIndex, lodNoDims, uv, stf).x;
+    }
+    else
+    {
+        if (mflags & RTXPT_MATFLAG_UseBaseOrDiffuseTexture) texBase = sampleMaterialTexture(sc, m.BaseOrDiffuseTextureIndex, lodNoDims, uv);
+        if (mflags & RTXPT_MATFLAG_UseEmissiveTexture) texEmissive = sampleMaterialTexture(sc, m.EmissiveTextureIndex, lodNoDims, uv);
+        if (mflags & RTXPT_MATFLAG_UseNormalTexture) texNormal = sampleMaterialTexture(sc, m.NormalTextureIndex, lodNoDims, uv);
+        if (mflags & RTXPT_MATFLAG_UseMetalRoughOrSpecularTexture) texMR = sampleMaterialTexture(sc, m.MetalRoughOrSpecularTextureIndex, lodNoDims, uv);
+        if (mflags & RTXPT_MATFLAG_UseTransmissionTexture) texTrans = sampleMaterialTexture(sc, m.TransmissionTextureIndex, lodNoDims, uv).x;
+    }
 
     const float3 matGeometryNormal = norm3(geometryNormal);
     float3 shadingNormal = matGeometryNormal;
@@ -520,7 +548,7 @@ PT_DEVICE void addFillSpecAvgChoice(uint& word, uint preFlags, uint preCounters)
 
 // MULTI: NEEFullSamples > 1 - the light samples' shadow records and the vertex's NEE block go straight to the launch's arrays (out.emitShadow stays false).  Without
 // NEE-AT feedback no draw depends on visibility, so the samples are drawn one after the other from the vertex's one uniform stream as HandleNEE draws them.
-template <bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, int MODE = kModeReference, bool NEEAT = false, bool MULTI = false, bool AMIS = false>
+template <bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, int MODE = kModeReference, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false>
 PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4 hit, HitOutputs& out)
 {
     out.continuePath = false; out.emitShadow = false;
@@ -545,7 +573,7 @@ PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4
 #ifdef PT_HOST_EMU
     emuLoadSurface(s);
 #else
-    loadSurface<MODE, AMIS>(p, __float_as_uint(hit.w), hit.y, hit.z, rayDir, path.coneWidth(), s, path.id, path.vertexIndex(), sampleIndex);
+    loadSurface<MODE, AMIS, STF>(p, __float_as_uint(hit.w), hit.y, hit.z, rayDir, path.coneWidth(), s, path.id, path.vertexIndex(), sampleIndex);
 #endif
     const uint ndq = p.c.nestedDielectricsQuality;
     if (ndq > 0 && path.interior0 != 0)

@@ -40,7 +40,8 @@ void launchInitTables(cudaStream_t s) { k_init_sobol_tables<<<16, 256, 0, s>>>()
 // ---- shade --------------------------------------------------------------------------------------------------------------------------------
 // MULTI (NEEFullSamples > 1): shadeHit appends the vertex's shadow records and NEE block itself, one record per valid light sample
 // AMIS: approximate light-vs-BSDF MIS (RtxptPathTracerConstants::useApproximateMIS = 1); a template argument, as RTXPT compiles it in
-template <int MINB, bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false>
+// STF: stochastic texture filtering of the material fetches (rtxpt_b200_set_texture_filtering); its kernels carry analytic lights, gated by the light type at run time
+template <int MINB, bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false>
 __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
@@ -63,7 +64,7 @@ __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ Lau
                 h = path.loadRay(p.stateIn, r, p.radiance);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
                 if (cls == 0) shadeMiss<EXPORT_GUIDES, kModeReference, NEEAT, AMIS>(p, path);
-                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT, MULTI, AMIS>(p, path, h, p.wf.hits[r], out);
+                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT, MULTI, AMIS, STF>(p, path, h, p.wf.hits[r], out);
                 path.storeRadiance(p.radiance, h);
                 if (out.continuePath) rayCls = 0;
                 if (out.emitShadow) shadowCls = 0;
@@ -115,6 +116,11 @@ __global__ void k_debug_rng(const uint* __restrict__ in, uint count, uint* __res
 // reference mode with NEE-AT feedback: one instantiation per MIS kind (guides on: the feedback passes reproject with them; analytic lights compiled in, gated by the light type at run time)
 void launchShadeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s)       // 3 CTAs per SM: 155 registers, no spills
 {
+    if (p.stf.pointTextures)
+    {
+        if (p.c.useApproximateMIS) k_shade<3, true, true, true, false, true, true><<<g.smCount * 3, 128, 0, s>>>(p); else k_shade<3, true, true, true, false, false, true><<<g.smCount * 3, 128, 0, s>>>(p);
+        return;
+    }
     if (p.c.useApproximateMIS) k_shade<3, true, true, true, false, true><<<g.smCount * 3, 128, 0, s>>>(p); else k_shade<3, true, true, true><<<g.smCount * 3, 128, 0, s>>>(p);
 }
 // the same choice of kernel for either MIS kind: the approximate kernels are the full-MIS ones with AMIS set
@@ -122,6 +128,14 @@ template <bool AMIS>
 static void launchShadeMis(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
 {
     const int grid = g.smCount * g.shadeBlocksPerSM;
+    if (p.stf.pointTextures)
+    {   // stochastic texture filtering: one kernel per guide / sample-count choice.  4 CTAs per SM although the single-sample kernels spill 12-24 bytes there: measured on an H100,
+        // k_shade on the bench workload is 7.37 ms at 4 CTAs and 7.76 ms at 3 without spills.  Like the guide and analytic-light kernels, they do not follow RTXPT_SHADE_CTAS
+        const bool multi = min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1;
+        if (multi) { if (p.exportGuides) k_shade<3, true, true, false, true, AMIS, true><<<g.smCount * 3, 128, 0, s>>>(p); else k_shade<3, false, true, false, true, AMIS, true><<<g.smCount * 3, 128, 0, s>>>(p); }
+        else { if (p.exportGuides) k_shade<4, true, true, false, false, AMIS, true><<<g.smCount * 4, 128, 0, s>>>(p); else k_shade<4, false, true, false, false, AMIS, true><<<g.smCount * 4, 128, 0, s>>>(p); }
+        return;
+    }
     // guide export and analytic (sphere) lights are separate instantiations: the default kernel carries neither
     if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1)
     {   // several light samples per vertex: analytic lights compiled in, gated by the light type at run time

@@ -122,8 +122,11 @@ struct LaunchParams
     // the set its continuing paths are appended to, and the radiance per home index h
     StateSet stateIn, stateOut;
     uint2* radiance;
+    // stochastic texture filtering (kernels instantiated with STF = true only; appended for the same reason): rtxpt_b200_set_texture_filtering's filter and sigma, and per bindless
+    // texture a point-filtered texture object over the same mip arrays and the texture's width, height and level count
+    struct { const cudaTextureObject_t* pointTextures; const uint4* textureDims; uint filterType; float sigma; } stf;
 };
-static_assert(sizeof(LaunchParams) == 1632, "the parameter block of every kernel keeps its layout");
+static_assert(sizeof(LaunchParams) == 1656, "the parameter block of every kernel keeps its layout");
 
 // ---- NEE blocks (NEEFullSamples = N > 1) ---------------------------------------------------------------------------------------------------------------
 // A vertex that takes light samples appends one block of 1 + N uint4 (counter kCtrNeeBlocks) to LaunchParams::neeBlocks: a header { path slot or home index h, the FILL

@@ -50,6 +50,7 @@ _SIGNATURES = {
     "rtxpt_b200_get_lights": [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)],
     "rtxpt_b200_set_view": [C.c_void_p, C.c_void_p],
     "rtxpt_b200_set_realtime": [C.c_void_p, C.POINTER(S.RealtimeConstants)],
+    "rtxpt_b200_set_texture_filtering": [C.c_void_p, C.POINTER(S.StochasticTextureFiltering)],
     "rtxpt_b200_path_trace_realtime": [C.c_void_p, C.c_int, C.c_void_p],
     "rtxpt_b200_denoiser_prepare_inputs": [C.c_void_p, C.c_uint32, C.c_int, C.POINTER(S.DenoiserConstants), C.c_void_p],
     "rtxpt_b200_denoiser_final_merge": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p],
@@ -334,6 +335,11 @@ class Context:
         return depth, mv, thp
 
     # ---- realtime mode (stable planes) ----
+    def set_texture_filtering(self, enable=True, filter_type=S.STF_FILTER_LINEAR, magnification_method=0, gaussian_sigma=0.3):
+        """Stochastic texture filtering of every material fetch (RTXPT's STFFilterMode / STFMagnificationMethod / STFGaussianSigma); raises and keeps the previous setting
+        when the description is refused"""
+        _check(self.L.rtxpt_b200_set_texture_filtering(self.h, C.byref(S.StochasticTextureFiltering(int(enable), filter_type, magnification_method, gaussian_sigma))), self.L)
+
     def set_realtime(self, rt):
         self.realtime = rt
         _check(self.L.rtxpt_b200_set_realtime(self.h, C.byref(rt)), self.L)

@@ -189,6 +189,14 @@ class EnvMapSceneParams(C.Structure):
     _fields_ = [("Transform", f32 * 12), ("InvTransform", f32 * 12), ("ColorMultiplier", f32 * 3), ("Enabled", f32)]
 
 
+class StochasticTextureFiltering(C.Structure):
+    """RtxptStochasticTextureFiltering (rtxpt_b200_set_texture_filtering): filterType STF_FILTER_TYPE_* (0 point, 1 linear, 2 cubic, 3 Gaussian), magnificationMethod 0 only"""
+    _fields_ = [("enable", u32), ("filterType", u32), ("magnificationMethod", u32), ("gaussianSigma", f32)]
+
+
+STF_FILTER_POINT, STF_FILTER_LINEAR, STF_FILTER_CUBIC, STF_FILTER_GAUSSIAN = 0, 1, 2, 3
+
+
 class PathTracerConstants(C.Structure):
     _fields_ = [("imageWidth", u32), ("imageHeight", u32), ("sampleBaseIndex", u32), ("perPixelJitterAAScale", f32),
                 ("bounceCount", u32), ("diffuseBounceCount", u32), ("EnvironmentMapDiffuseSampleMIPLevel", f32), ("texLODBias", f32),
