@@ -316,6 +316,67 @@ typedef struct RtxptStochasticTextureFiltering {
 #define RTXPT_STF_FILTER_TYPE_GAUSSIAN  3u
 RTXPT_API int rtxpt_b200_set_texture_filtering(rtxpt_ctx* ctx, const RtxptStochasticTextureFiltering* stf);
 
+/* Debug views (RTXPT's m_ui.DebugView -> DebugConstants::debugViewType, DebugViewType in Rtxpt/Shaders/PathTracer/PathTracerDebug.hlsli:25-65; m_ui.DebugViewStablePlaneIndex ->
+ * debugViewStablePlaneIndex, Sample.cpp:2160-2161).  A view other than DISABLED makes every path_trace / path_trace_realtime call first clear RTXPT_BUFFER_DEBUG_VIZ_F16 (RGBA16F,
+ * width x height, allocated by the first such call; RTXPT's u_ShaderDebugVizTextureBuffer, which RTXPT clears when the accumulation restarts, Sample.cpp:1427) and then draw the view into it.  Drawing the
+ * buffer over the output colour (RTXPT blends it over ProcessedOutputColor) is the host's job.  Nothing else a call computes changes with the view.
+ *   FIRST_HIT_*:     surfaceDebugViz (PathTracerBridgeDonut.hlsli:457-510) at path vertex 1: in reference mode of the last sub-sample of the call (only the call's last launch
+ *                    draws), in realtime mode of the BUILD pass.  Pixels whose camera ray misses keep the cleared value.  The shader ID is 0xFFFFFFFF for every surface (one
+ *                    shader; RTXPT without RTXPT_SHADER_ID)
+ *   DOMINANT_STABLE_PLANE_INDEX, STABLE_PLANE_VIRTUAL_RAY_LENGTH .. STABLE_PLANE_SPEC_RADIANCE, STABLE_RADIANCE: StablePlanesDebugViz (PathTracerDebug.hlsli:359-461) after the
+ *                    FILL passes of path_trace_realtime; nothing is drawn in reference mode, which has no stable planes (Sample.cpp:2551).  The mouse crosshair is not drawn
+ *   STABLE_PLANE_RELAXED_DISOCCLUSION .. STABLE_PLANE_DENOISER_VALIDATION: DENOISER_FINAL_MERGE's views (PostProcess.hlsl:633-681), drawn by rtxpt_b200_denoiser_final_merge
+ *                    (and so by rtxpt_b200_denoise_realtime) for the plane it merges.  With the split, of the four pixels that land on one quadrant pixel the one of even
+ *                    coordinates draws (RTXPT leaves it to the GPU).  NRD's validation layer is not part of this library: DENOISER_VALIDATION shows the combined denoised radiance
+ *   stablePlaneIndex: 0..2 shows that plane, RTXPT_DEBUG_VIEW_STABLE_PLANE_SPLIT (-1 in RTXPT) the three planes in four half-resolution quadrants; with one active plane
+ *                    plane 0 is shown, as Sample.cpp:2161 does.  Any other value is RTXPT_ERR_INVALID_ARGUMENT
+ * Refused with RTXPT_ERR_UNSUPPORTED: DENOISER_GUIDE_* (the DLSS-RR guide buffers), VBUFFER_*, SECONDARY_SURFACE_*, RESTIR*, REGIR_* (RTXDI and the raster V-buffer, which this library does not have).  debugViewType >= RTXPT_DEBUG_VIEW_MAX_COUNT
+ * is RTXPT_ERR_INVALID_ARGUMENT.  A refused description leaves the context's view as it was.  Applies from the next path_trace / path_trace_realtime. */
+typedef struct RtxptDebugView {
+    uint32_t debugViewType;                 /* RTXPT_DEBUG_VIEW_* */
+    uint32_t stablePlaneIndex;
+} RtxptDebugView;
+#define RTXPT_DEBUG_VIEW_DISABLED                           0u
+#define RTXPT_DEBUG_VIEW_DOMINANT_STABLE_PLANE_INDEX        1u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_VIRTUAL_RAY_LENGTH    2u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_MOTION_VECTORS        3u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_NORMALS               4u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_ROUGHNESS             5u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_SPEC_AVG              6u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_DIFF_BSDF_ESTIMATE    7u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_DIFF_RADIANCE         8u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_SPEC_BSDF_ESTIMATE    9u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_SPEC_RADIANCE         10u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_RELAXED_DISOCCLUSION  11u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_DIFF_RADIANCE_DENOISED 12u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_SPEC_RADIANCE_DENOISED 13u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_COMBINED_RADIANCE_DENOISED 14u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_VIEW_Z                15u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_THROUGHPUT            16u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_DENOISER_VALIDATION   17u
+#define RTXPT_DEBUG_VIEW_STABLE_RADIANCE                    18u
+#define RTXPT_DEBUG_VIEW_DENOISER_GUIDE_DEPTH               19u     /* .. DENOISER_GUIDE_PRIMARY_LAYER 28 */
+#define RTXPT_DEBUG_VIEW_DENOISER_GUIDE_PRIMARY_LAYER       28u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_BARYCENTRICS             29u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_FACE_NORMAL              30u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_GEOMETRY_NORMAL          31u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_SHADING_NORMAL           32u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_SHADING_TANGENT          33u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_SHADING_BITANGENT        34u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_FRONT_FACING             35u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_THIN_SURFACE             36u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_DIFFUSE                  37u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_SPECULAR                 38u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_ROUGHNESS                39u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_METALLIC                 40u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_SHADER_ID                41u
+#define RTXPT_DEBUG_VIEW_FIRST_HIT_MATERIAL_ID              42u
+#define RTXPT_DEBUG_VIEW_VBUFFER_MOTION_VECTORS             43u     /* .. REGIR_INDIRECT_OUTPUT 53 */
+#define RTXPT_DEBUG_VIEW_REGIR_INDIRECT_OUTPUT              53u
+#define RTXPT_DEBUG_VIEW_MAX_COUNT                          54u
+#define RTXPT_DEBUG_VIEW_STABLE_PLANE_SPLIT                 0xFFFFFFFFu
+RTXPT_API int rtxpt_b200_set_debug_view(rtxpt_ctx* ctx, const RtxptDebugView* view);
+
 /* Replaces the loop body of Sample::PathTrace (Rtxpt/Sample.cpp:2503-2517): setPushConstants({subSampleIndex}) +
  * dispatchRays(width,height), for subSampleCount consecutive sub-samples starting at firstSubSampleIndex, each followed
  * by the reference-mode accumulation (AccumulationPass::Render, Rtxpt/Sample.cpp:2770-2778) when accumulate != 0.
@@ -616,6 +677,7 @@ RTXPT_API int rtxpt_b200_unpack_all(rtxpt_ctx* ctx, const void* dSrcAll, void* c
  * tileWorld x that many bytes, rtxpt_b200_exchange_unpack.  With NEEATFeedback = 0 the assembled frame is bit-identical to the single-GPU frame (tests/test_gpu_multi.py); with
  * feedback every rank adapts on its own tiles (independent global tables, local samplers clamped at screen-tile borders: still unbiased, SURVEY §8e). */
 enum { RTXPT_BUFFER_STABLE_PLANE_NEIGHBOUR_GUIDES = 20 };     /* exchange only: per plane { branch ID, StablePlane::PackedNormal } of every pixel */
+enum { RTXPT_BUFFER_DEBUG_VIZ_F16 = 21 };     /* RGBA16F debug view (rtxpt_b200_set_debug_view); RTXPT_ERR_INVALID_ARGUMENT until a call with a view has allocated it */
 RTXPT_API int rtxpt_b200_exchange_bytes(rtxpt_ctx* ctx, const int* buffers, uint32_t count, size_t* outBytesPerRank);
 RTXPT_API int rtxpt_b200_exchange_pack(rtxpt_ctx* ctx, const int* buffers, uint32_t count, void* dDst, void* cudaStream);
 RTXPT_API int rtxpt_b200_exchange_unpack(rtxpt_ctx* ctx, const int* buffers, uint32_t count, const void* dSrcAllRanks, void* cudaStream);

@@ -4,6 +4,7 @@
 // structure build, MaterialsBaker::Update, UpdateLighting, constant-buffer write, PathTrace, AccumulationPass.
 // There is no CPU rendering fallback anywhere in this library: without a CUDA device every entry point fails with RTXPT_ERR_NO_DEVICE.
 #include "kernels.h"
+#include "debug_views.cuh"
 #include "opacity_masks.h"
 #include "reblur_host.h"
 #include "neeat_host.h"
@@ -117,6 +118,7 @@ struct rtxpt_ctx
     std::vector<DeviceTexture> textures; DeviceArray<cudaTextureObject_t> dTextureTable;
     DeviceArray<cudaTextureObject_t> dPointTextureTable; DeviceArray<uint4> dTextureDims;     // stochastic texture filtering: point-filtered objects, width / height / levels
     RtxptStochasticTextureFiltering stf{};                                                  // rtxpt_b200_set_texture_filtering (off)
+    RtxptDebugView debugView{}; DeviceArray<uint2> debugViz;                                 // rtxpt_b200_set_debug_view (disabled); RGBA16F, allocated by the first call that draws
     DeviceTexture envCube; uint32_t envFaceSize = 0, envMipLevels = 0;
     // rtxpt_b200_update_env_map: the bake's linear MIP chain and the importance map's, grown to the largest cube baked and never shrunk; the source of the last update, kept so
     // that the next update can re-bake from it; event times of the last update (bake, importance map, copy into the cube, readback + light bake + upload)
@@ -666,6 +668,31 @@ extern "C" RTXPT_API int rtxpt_b200_set_texture_filtering(rtxpt_ctx* c, const Rt
     return RTXPT_OK;
 }
 
+extern "C" RTXPT_API int rtxpt_b200_set_debug_view(rtxpt_ctx* c, const RtxptDebugView* v)
+{
+    if (!c || !v) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    const uint32_t t = v->debugViewType;
+    if (t >= RTXPT_DEBUG_VIEW_MAX_COUNT) return fail(RTXPT_ERR_INVALID_ARGUMENT, "debugViewType %u: DebugViewType has %u values", t, RTXPT_DEBUG_VIEW_MAX_COUNT);
+    if (v->stablePlaneIndex >= RTXPT_STABLE_PLANE_COUNT && v->stablePlaneIndex != RTXPT_DEBUG_VIEW_STABLE_PLANE_SPLIT)
+        return fail(RTXPT_ERR_INVALID_ARGUMENT, "stablePlaneIndex %u: 0..2 or RTXPT_DEBUG_VIEW_STABLE_PLANE_SPLIT", v->stablePlaneIndex);
+    if (t >= RTXPT_DEBUG_VIEW_DENOISER_GUIDE_DEPTH && t <= RTXPT_DEBUG_VIEW_DENOISER_GUIDE_PRIMARY_LAYER)
+        return fail(RTXPT_ERR_UNSUPPORTED, "debugViewType %u: the DenoiserGuide views read the DLSS-RR guide buffers, which this library does not produce", t);
+    if (t >= RTXPT_DEBUG_VIEW_VBUFFER_MOTION_VECTORS)
+        return fail(RTXPT_ERR_UNSUPPORTED, "debugViewType %u: the V-buffer, secondary-surface, ReSTIR and ReGIR views belong to RTXDI and the raster V-buffer, which this library does not have", t);
+    c->debugView = *v;
+    return RTXPT_OK;
+}
+// a call that draws a debug view starts from a cleared target.  RTXPT clears u_ShaderDebugVizTextureBuffer when the accumulation restarts (Sample.cpp:1427, under resetAccum);
+// clearing on every call keeps a view from showing what an earlier call drew
+static int clearDebugViz(rtxpt_ctx* c, cudaStream_t s)
+{
+    if (c->debugView.debugViewType == RTXPT_DEBUG_VIEW_DISABLED) return RTXPT_OK;
+    const size_t P = size_t(c->tableWidth) * c->tableHeight;
+    if (c->debugViz.count != P) { CU(syncContext(c)); CU(c->debugViz.alloc(P)); }
+    CU(cudaMemsetAsync(c->debugViz.ptr, 0, P * sizeof(uint2), s));
+    return RTXPT_OK;
+}
+
 // ---- launch --------------------------------------------------------------------------------------------------------------------------------
 static void fillParams(rtxpt_ctx* c, LaunchParams& p)
 {
@@ -687,6 +714,11 @@ static void fillParams(rtxpt_ctx* c, LaunchParams& p)
     if (c->stf.enable && c->dPointTextureTable.ptr)
     {   // stochastic texture filtering: the launchers pick the STF kernels when the table is set
         p.stf.pointTextures = c->dPointTextureTable.ptr; p.stf.textureDims = c->dTextureDims.ptr; p.stf.filterType = c->stf.filterType; p.stf.sigma = c->stf.gaussianSigma;
+    }
+    if (c->debugView.debugViewType != RTXPT_DEBUG_VIEW_DISABLED)
+    {   // the launchers pick the debug-view kernels when the target is set; one active plane shows plane 0 (Sample.cpp:2161)
+        p.dbg.viz = c->debugViz.ptr; p.dbg.view = c->debugView.debugViewType;
+        p.dbg.planeIndex = (c->haveRealtime && c->realtime.activeStablePlaneCount == 1) ? 0 : int(c->debugView.stablePlaneIndex);
     }
     p.c = c->consts;
     p.flags = c->cfg.flags;
@@ -772,6 +804,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
     // tile partition (tileWorld > 1) with feedback: every rank adapts on the tiles it owns - independent global tables, reservoirs of foreign pixels stay empty (SURVEY §8e)
     if (na && !(c->cfg.flags & RTXPT_CFG_EXPORT_GUIDES)) return fail(RTXPT_ERR_INVALID_ARGUMENT, "NEE-AT feedback in reference mode reprojects with the exported guides: create the context with RTXPT_CFG_EXPORT_GUIDES");
     cudaStream_t s = pickStream(c, cudaStream);
+    rc = clearDebugViz(c, s); if (rc != RTXPT_OK) return rc;
     LaunchParams p; fillParams(c, p);
     if (na)
     {
@@ -820,7 +853,8 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace(rtxpt_ctx* c, uint32_t firstSubSa
             q.firstSampleIndex = c->consts.sampleBaseIndex + firstSubSampleIndex + done + firstSub;
             q.subSampleCount = count;
             q.accumulatedSamples = c->accumulatedSamples + firstSub; q.doAccumulate = accumulate ? 1u : 0u;
-            if (l + 1 != lanes) q.exportGuides = 0;     // the guides hold the launch's last sub-sample, as after the reference's sequential dispatches
+            if (l + 1 != lanes) { q.exportGuides = 0; q.dbg.viz = nullptr; }     // the guides and the first-hit debug view hold the launch's last sub-sample, as after the reference's sequential dispatches
+            if (done + n != subSampleCount) q.dbg.viz = nullptr;                  // the first-hit debug view holds the call's last sub-sample, whatever the launch split
             q.iteration = 0;
             KernelTimer ktl{ c, ls, kt.on };
             ktl.begin(3); launchGenerate(q, c->grid, ls); ktl.end(); launches++;
@@ -918,6 +952,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
     if (na && (!c->na.allocated || !c->na.frameBegun)) return fail(RTXPT_ERR_INVALID_ARGUMENT, "NEEATFeedback is set: call rtxpt_b200_neeat_update_begin before tracing the frame");
     const bool multi = neeFullSamples(c) > 1;
     if (multi) { rc = ensureNeeSamples(c); if (rc != RTXPT_OK) return rc; }
+    rc = clearDebugViz(c, s); if (rc != RTXPT_OK) return rc;
     LaunchParams p; fillParams(c, p);
     const RtxptRealtimeConstants& r = c->realtime;
     fillRealtimeParams(c, p);
@@ -968,6 +1003,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
         }
         launchRtFillCommit(p, c->grid, s); launches++;
     }
+    if (p.dbg.viz && isStablePlaneView(p.dbg.view)) { launchRtDebugViz(p, c->grid, s); launches++; }      // StablePlanesDebugViz after the FILL pass (Sample.cpp:2551-2555)
     if (mergeNoDenoiser) { launchRtMerge(p, c->grid, s); launches++; }
     CU(cudaGetLastError());
     CU(cudaEventRecord(c->evStop, s));
@@ -1654,6 +1690,9 @@ static int targetInfo(rtxpt_ctx* c, int buffer, void** ptr, size_t* bytes)
         default: *ptr = c->dnHistoryClampRelax.ptr; *bytes = P; break;
         }
         return RTXPT_OK;
+    case RTXPT_BUFFER_DEBUG_VIZ_F16:
+        if (c->debugViz.count != P) return fail(RTXPT_ERR_INVALID_ARGUMENT, "the debug view target does not exist before a path_trace call with a debug view set");
+        *ptr = c->debugViz.ptr; *bytes = P * 8; return RTXPT_OK;
     case RTXPT_BUFFER_LDR_COLOR_RGBA8:
         if (!c->toneMapped || c->ldrColor.count != P) return fail(RTXPT_ERR_INVALID_ARGUMENT, "the LDR colour does not exist before rtxpt_b200_tone_map");
         *ptr = c->ldrColor.ptr; *bytes = P * 4; return RTXPT_OK;

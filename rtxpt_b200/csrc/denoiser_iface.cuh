@@ -3,6 +3,7 @@
 // :646-677, :728-750, :869-874).  Kernels: realtime_kernels.cu; host build for the CPU parity test: tests/emu.
 #pragma once
 #include "wavefront.cuh"
+#include "debug_views.cuh"
 
 namespace pt {
 
@@ -125,5 +126,31 @@ PT_HD void dnFinalMergePixel(const LaunchParams& p, const uint id)
         const uint2 c = p.outputColor[o];
         p.outputColor[o] = make_uint2(f32tof16(f16tof32(c.x) + sum.x) | (f32tof16(f16tof32(c.x >> 16) + sum.y) << 16), f32tof16(f16tof32(c.y) + sum.z) | (c.y & 0xFFFF0000u));
     }
+
+// the denoiser-merge debug views of the merged plane (PostProcess.hlsl:633-681, rtxpt_b200_set_debug_view): the same inputs as dnFinalMergePixel, read again
+PT_HD void dnFinalMergeDebugPixel(const LaunchParams& p, const uint id)
+{
+    const uint px = id >> 16, py = id & 0xFFFFu, W = p.c.imageWidth, H = p.c.imageHeight;
+    const size_t o = pixelOffset(p, id);
+    const uint4* rec = reinterpret_cast<const uint4*>(p.rt.planes + planeAddress(p.rt, id, p.rt.dnPlane));
+    if (mergeDebugChecker(p.dbg.planeIndex, p.rt.dnPlane, px, py, W, H, p.rt.activePlaneCount)) { const float c = float((px + py) % 2u); p.dbg.viz[o] = packDebugPixel(make_float4(c, c, c, 1.0f)); }
+    uint tx, ty;
+    if (!mergeDebugTarget(p.dbg.view, p.dbg.planeIndex, p.rt.dnPlane, px, py, W, H, tx, ty)) return;
+    MergeDebugInputs m;
+    m.viewZ = p.rt.dnViewZ[o];
+    m.relaxedDisocclusion = 0.0f; m.diff = mk3(0.0f); m.spec = mk3(0.0f);
+    if (m.viewZ != 3.402823466e+38f)
+    {
+        const uint4 r3 = rec[3];
+        const float3 diffEstimate = mk3(f16tof32(r3.x >> 16), f16tof32(r3.y >> 16), f16tof32(r3.z >> 16)), specEstimate = mk3(f16tof32(r3.x), f16tof32(r3.y), f16tof32(r3.z));
+        const uint2 dd = p.rt.dnDenoisedDiff[o], ds = p.rt.dnDenoisedSpec[o];
+        m.diff = yCoCgToLinear(mk3(f16tof32(dd.x), f16tof32(dd.x >> 16), f16tof32(dd.y))) * diffEstimate;
+        m.spec = yCoCgToLinear(mk3(f16tof32(ds.x), f16tof32(ds.x >> 16), f16tof32(ds.y))) * specEstimate;
+        m.relaxedDisocclusion = float(p.rt.dnDisocclusionMix[o]) / 255.0f;             // R8_UNORM
+    }
+    const uint4 r2 = rec[2];                                                              // PackedThpAndMVs: throughput in the high halves
+    m.throughput = mk3(f16tof32(r2.x >> 16), f16tof32(r2.y >> 16), f16tof32(r2.z >> 16));
+    p.dbg.viz[size_t(ty) * W + tx] = packDebugPixel(mergeDebugColor(p.dbg.view, m));
+}
 
 } // namespace pt

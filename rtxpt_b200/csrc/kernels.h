@@ -27,6 +27,7 @@ void launchRtFillGenerate(const LaunchParams& p, const GridConfig& g, cudaStream
 void launchRtShade(const LaunchParams& p, const GridConfig& g, bool fill, cudaStream_t s);
 void launchRtFillCommit(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
+void launchRtDebugViz(const LaunchParams& p, const GridConfig& g, cudaStream_t s);          // StablePlanesDebugViz after the FILL passes (rtxpt_b200_set_debug_view)
 void launchDnPrepareInputs(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchDnFinalMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchCommitAccumulate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);

@@ -125,7 +125,8 @@ __global__ void __launch_bounds__(256) k_rt_fill_generate(const __grid_constant_
 // MULTI (FILL pass, NEEFullSamples > 1): shadeHit appends the vertex's shadow records and NEE block itself, one record per valid light sample; 3 CTAs per SM, which
 // lets it run without spills in both builds.  AMIS (FILL pass): approximate light-vs-BSDF MIS; the BUILD pass evaluates no MIS (PathState.hlsli:157-159) and has one kernel for both kinds
 // STF: stochastic texture filtering of the material fetches (rtxpt_b200_set_texture_filtering); its kernels carry analytic lights, gated by the light type at run time
-template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false>
+// DEBUG_VIEW (BUILD pass): a first-hit debug view is set (rtxpt_b200_set_debug_view); its kernels carry analytic lights, gated by the light type at run time
+template <int MODE, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false, bool DEBUG_VIEW = false>
 __global__ void __launch_bounds__(128, (MULTI || STF) ? 3 : PT_RT_SHADE_CTAS) k_rt_shade(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
@@ -148,7 +149,7 @@ __global__ void __launch_bounds__(128, (MULTI || STF) ? 3 : PT_RT_SHADE_CTAS) k_
                 PathRegs path; path.load(p.wf, slot, true);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
                 if (cls == 0) shadeMiss<false, MODE, NEEAT, AMIS>(p, path);
-                else shadeHit<false, ANALYTIC_LIGHTS, MODE, NEEAT, MULTI, AMIS, STF>(p, path, slot, p.wf.hits[slot], out);
+                else shadeHit<false, ANALYTIC_LIGHTS, MODE, NEEAT, MULTI, AMIS, STF, DEBUG_VIEW>(p, path, slot, p.wf.hits[slot], out);
                 continues = (cls != 0) && out.continuePath;
                 if constexpr (MODE == kModeBuildStablePlanes)
                 {   // postProcessHit: when this branch has ended, continue with the next enqueued branch of the pixel (planes above the current one)
@@ -206,14 +207,40 @@ __global__ void __launch_bounds__(256) k_rt_merge(const __grid_constant__ Launch
     }
 }
 
+// ---- StablePlanesDebugViz (PathTracerDebug.hlsli:359-461), run after the FILL passes (Sample.cpp:2551-2555): one thread per pixel of the context ---------------------------
+struct DebugVizBuffers
+{
+    const LaunchParams& p;
+    __device__ uint branchID(uint x, uint y, uint plane) const { return headerWord(p, (x << 16) | y, plane); }
+    __device__ RtxptStablePlane plane(uint x, uint y, uint plane) const { return p.rt.planes[planeAddress(p.rt, (x << 16) | y, plane)]; }
+    __device__ uint dominantIndex(uint x, uint y) const { return headerWord(p, (x << 16) | y, 3) & 3u; }
+    __device__ float3 stableRadiance(uint x, uint y) const { const uint2 r = p.rt.stableRadiance[size_t(y) * p.c.imageWidth + x]; return mk3(f16tof32(r.x), f16tof32(r.x >> 16), f16tof32(r.y)); }
+};
+__global__ void __launch_bounds__(256) k_rt_debug_viz(const __grid_constant__ LaunchParams p)
+{
+    const DebugVizBuffers buffers{ p };
+    for (uint slot = blockIdx.x * blockDim.x + threadIdx.x; slot < p.wf.pixelCount; slot += gridDim.x * blockDim.x)
+    {
+        const uint id = p.wf.pixelOfSlot[slot];
+        const float4 c = stablePlaneDebugPixel(p.dbg.view, p.dbg.planeIndex, id >> 16, id & 0xFFFFu, p.c.imageWidth, p.c.imageHeight, buffers);      // the split reads other pixels' planes
+        if (c.w > 0.0f) p.dbg.viz[pixelOffset(p, id)] = packDebugPixel(c);
+    }
+}
+
 // ---- RTXPT's side of the denoiser interface (SURVEY §8 row a18): bodies in denoiser_iface.cuh ----
 __global__ void __launch_bounds__(256) k_dn_prepare_inputs(const __grid_constant__ LaunchParams p)
 {
     for (uint slot = blockIdx.x * blockDim.x + threadIdx.x; slot < p.wf.pixelCount; slot += gridDim.x * blockDim.x) dnPrepareInputsPixel(p, p.wf.pixelOfSlot[slot]);
 }
+// DEBUG_VIEW: a denoiser-merge debug view is set (rtxpt_b200_set_debug_view); the merge also draws it
+template <bool DEBUG_VIEW = false>
 __global__ void __launch_bounds__(256) k_dn_final_merge(const __grid_constant__ LaunchParams p)
 {
-    for (uint slot = blockIdx.x * blockDim.x + threadIdx.x; slot < p.wf.pixelCount; slot += gridDim.x * blockDim.x) dnFinalMergePixel(p, p.wf.pixelOfSlot[slot]);
+    for (uint slot = blockIdx.x * blockDim.x + threadIdx.x; slot < p.wf.pixelCount; slot += gridDim.x * blockDim.x)
+    {
+        dnFinalMergePixel(p, p.wf.pixelOfSlot[slot]);
+        if constexpr (DEBUG_VIEW) dnFinalMergeDebugPixel(p, p.wf.pixelOfSlot[slot]);
+    }
 }
 // DenoiseSpecHitT: one thread per pixel over the full frame (row-major guides); src / dst alternate between the guide and a scratch image
 __global__ void __launch_bounds__(256) k_dn_spec_hitt(const float* __restrict__ src, const float* __restrict__ depth, float* __restrict__ dst, int W, int H)
@@ -256,7 +283,10 @@ void launchRtUnpackPlaneGuides(const LaunchParams& p, const uint32_t* allPixelTa
 { k_rt_unpack_plane_guides<<<g.smCount * 4, 256, 0, s>>>(p, allPixelTable, paddedCount, world, skipRank, static_cast<const uint8_t*>(srcAll), segmentOffset, bytesPerRank); }
 void launchDnSpecHitT(const float* src, const float* depth, float* dst, int W, int H, cudaStream_t s) { k_dn_spec_hitt<<<dim3((W + 15) / 16, (H + 15) / 16), dim3(16, 16), 0, s>>>(src, depth, dst, W, H); }
 void launchDnPrepareInputs(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_dn_prepare_inputs<<<g.smCount * 4, 256, 0, s>>>(p); }
-void launchDnFinalMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_dn_final_merge<<<g.smCount * 4, 256, 0, s>>>(p); }
+void launchDnFinalMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
+{
+    if (p.dbg.viz && isDenoiserMergeView(p.dbg.view)) k_dn_final_merge<true><<<g.smCount * 4, 256, 0, s>>>(p); else k_dn_final_merge<<<g.smCount * 4, 256, 0, s>>>(p);
+}
 
 void launchRtBuildGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_build_generate<<<g.smCount * 4, 256, 0, s>>>(p); }
 void launchRtFillGenerate(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_fill_generate<<<g.smCount * 4, 256, 0, s>>>(p); }
@@ -287,6 +317,12 @@ static void launchRtShadeFill(const LaunchParams& p, const GridConfig& g, cudaSt
 void launchRtShade(const LaunchParams& p, const GridConfig& g, bool fill, cudaStream_t s)
 {
     const int grid = g.smCount * PT_RT_SHADE_CTAS;
+    if (!fill && p.dbg.viz && isFirstHitView(p.dbg.view))
+    {   // first-hit debug view: drawn by the BUILD pass, whose vertex 1 is the camera ray's hit
+        if (p.stf.pointTextures) k_rt_shade<kModeBuildStablePlanes, true, false, false, false, true, true><<<g.smCount * 3, 128, 0, s>>>(p);
+        else k_rt_shade<kModeBuildStablePlanes, true, false, false, false, false, true><<<grid, 128, 0, s>>>(p);
+        return;
+    }
     if (!fill && p.stf.pointTextures) { k_rt_shade<kModeBuildStablePlanes, true, false, false, false, true><<<g.smCount * 3, 128, 0, s>>>(p); return; }
     if (!fill) { if (p.scene.analyticLightCount != 0) k_rt_shade<kModeBuildStablePlanes, true><<<grid, 128, 0, s>>>(p); else k_rt_shade<kModeBuildStablePlanes, false><<<grid, 128, 0, s>>>(p); }
     else if (p.c.useApproximateMIS) launchRtShadeFill<true>(p, g, s);
@@ -294,5 +330,6 @@ void launchRtShade(const LaunchParams& p, const GridConfig& g, bool fill, cudaSt
 }
 void launchRtFillCommit(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_fill_commit<<<g.smCount * 4, 256, 0, s>>>(p); }
 void launchRtMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_merge<<<g.smCount * 4, 256, 0, s>>>(p); }
+void launchRtDebugViz(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_rt_debug_viz<<<g.smCount * 4, 256, 0, s>>>(p); }
 
 } // namespace pt

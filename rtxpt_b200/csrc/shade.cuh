@@ -19,6 +19,7 @@
 #include "wavefront.cuh"
 #include "bsdf.cuh"
 #include "stf.cuh"
+#include "debug_views.cuh"
 
 namespace pt {
 
@@ -546,9 +547,22 @@ PT_DEVICE void addFillSpecAvgChoice(uint& word, uint preFlags, uint preCounters)
     }
 }
 
+// surfaceDebugViz (PathTracerBridgeDonut.hlsli:457-510, called at the end of Bridge::loadSurface): the first-hit debug view from the surface just loaded
+PT_DEVICE void storeFirstHitDebugView(const LaunchParams& p, uint id, float bu, float bv, const Surface& s)
+{
+    FirstHitDebugInputs d;
+    d.barycentrics = mk2(bu, bv);
+    d.faceN = s.faceN; d.vertexN = s.vertexN; d.N = s.N; d.T = s.T; d.B = s.B;
+    d.frontFacing = s.frontFacing; d.thin = s.thin;
+    d.diffuse = s.bsdf.diffuse; d.specular = s.bsdf.specular; d.roughness = s.bsdf.roughness; d.metallic = s.bsdf.metallic;
+    d.materialID = s.materialID;
+    p.dbg.viz[pixelOffset(p, id)] = packDebugPixel(firstHitDebugColor(p.dbg.view, d));
+}
+
 // MULTI: NEEFullSamples > 1 - the light samples' shadow records and the vertex's NEE block go straight to the launch's arrays (out.emitShadow stays false).  Without
 // NEE-AT feedback no draw depends on visibility, so the samples are drawn one after the other from the vertex's one uniform stream as HandleNEE draws them.
-template <bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, int MODE = kModeReference, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false>
+// DEBUG_VIEW: a first-hit debug view is set (LaunchParams::dbg); vertex 1 draws it - in reference mode only in the call's last sub-sample, whose value RTXPT's last dispatch leaves
+template <bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, int MODE = kModeReference, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false, bool DEBUG_VIEW = false>
 PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4 hit, HitOutputs& out)
 {
     out.continuePath = false; out.emitShadow = false;
@@ -575,6 +589,8 @@ PT_DEVICE void shadeHit(const LaunchParams& p, PathRegs& path, uint slot, float4
 #else
     loadSurface<MODE, AMIS, STF>(p, __float_as_uint(hit.w), hit.y, hit.z, rayDir, path.coneWidth(), s, path.id, path.vertexIndex(), sampleIndex);
 #endif
+    if constexpr (DEBUG_VIEW)
+        if (path.vertexIndex() == 1 && (MODE != kModeReference || path.sampleIndex + 1 == p.firstSampleIndex + p.subSampleCount)) storeFirstHitDebugView(p, path.id, hit.y, hit.z, s);
     const uint ndq = p.c.nestedDielectricsQuality;
     if (ndq > 0 && path.interior0 != 0)
     {   // homogeneous absorption through the medium we are in (PathTracer.hlsli:538-547, BridgeDonut:871-887)

@@ -41,7 +41,8 @@ void launchInitTables(cudaStream_t s) { k_init_sobol_tables<<<16, 256, 0, s>>>()
 // MULTI (NEEFullSamples > 1): shadeHit appends the vertex's shadow records and NEE block itself, one record per valid light sample
 // AMIS: approximate light-vs-BSDF MIS (RtxptPathTracerConstants::useApproximateMIS = 1); a template argument, as RTXPT compiles it in
 // STF: stochastic texture filtering of the material fetches (rtxpt_b200_set_texture_filtering); its kernels carry analytic lights, gated by the light type at run time
-template <int MINB, bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false>
+// DEBUG_VIEW: a first-hit debug view is set (rtxpt_b200_set_debug_view); its kernels carry analytic lights, gated by the light type at run time
+template <int MINB, bool EXPORT_GUIDES, bool ANALYTIC_LIGHTS, bool NEEAT = false, bool MULTI = false, bool AMIS = false, bool STF = false, bool DEBUG_VIEW = false>
 __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ LaunchParams p)
 {
     uint* ctr = p.wf.counters + p.iteration * kCountersPerIter;
@@ -64,7 +65,7 @@ __global__ void __launch_bounds__(128, MINB) k_shade(const __grid_constant__ Lau
                 h = path.loadRay(p.stateIn, r, p.radiance);
                 if constexpr (NEEAT) out.naRecord = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
                 if (cls == 0) shadeMiss<EXPORT_GUIDES, kModeReference, NEEAT, AMIS>(p, path);
-                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT, MULTI, AMIS, STF>(p, path, h, p.wf.hits[r], out);
+                else shadeHit<EXPORT_GUIDES, ANALYTIC_LIGHTS, kModeReference, NEEAT, MULTI, AMIS, STF, DEBUG_VIEW>(p, path, h, p.wf.hits[r], out);
                 path.storeRadiance(p.radiance, h);
                 if (out.continuePath) rayCls = 0;
                 if (out.emitShadow) shadowCls = 0;
@@ -113,9 +114,27 @@ __global__ void k_debug_rng(const uint* __restrict__ in, uint count, uint* __res
     for (uint k = 0; k < 4; k++) out[i * 8 + 4 + k] = __float_as_uint(hashToFloat(ldSampleBits(baseHash, in[i * 4 + 3], 1u, k)));
 }
 
+// first-hit debug view: the kernel the launch would run otherwise, with the view drawn at vertex 1; one instantiation per guide / sample-count / STF choice, analytic lights
+// gated at run time, at the CTA count of the kernel it stands in for
+template <int MINB, bool EXPORT_GUIDES, bool NEEAT, bool MULTI, bool AMIS, bool STF>
+static void launchShadeDebugView(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_shade<MINB, EXPORT_GUIDES, true, NEEAT, MULTI, AMIS, STF, true><<<g.smCount * MINB, 128, 0, s>>>(p); }
+template <bool AMIS, bool STF>
+static void launchShadeDebugViewMis(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
+{
+    if (min(kNeeMaxFullSamples, p.c.NEEFullSamples) > 1) { if (p.exportGuides) launchShadeDebugView<3, true, false, true, AMIS, STF>(p, g, s); else launchShadeDebugView<3, false, false, true, AMIS, STF>(p, g, s); }
+    else { if (p.exportGuides) launchShadeDebugView<4, true, false, false, AMIS, STF>(p, g, s); else launchShadeDebugView<4, false, false, false, AMIS, STF>(p, g, s); }
+}
+static bool firstHitDebugView(const LaunchParams& p) { return p.dbg.viz && isFirstHitView(p.dbg.view); }
+
 // reference mode with NEE-AT feedback: one instantiation per MIS kind (guides on: the feedback passes reproject with them; analytic lights compiled in, gated by the light type at run time)
 void launchShadeNeeat(const LaunchParams& p, const GridConfig& g, cudaStream_t s)       // 3 CTAs per SM: 155 registers, no spills
 {
+    if (firstHitDebugView(p))
+    {
+        if (p.stf.pointTextures) { if (p.c.useApproximateMIS) launchShadeDebugView<3, true, true, false, true, true>(p, g, s); else launchShadeDebugView<3, true, true, false, false, true>(p, g, s); }
+        else { if (p.c.useApproximateMIS) launchShadeDebugView<3, true, true, false, true, false>(p, g, s); else launchShadeDebugView<3, true, true, false, false, false>(p, g, s); }
+        return;
+    }
     if (p.stf.pointTextures)
     {
         if (p.c.useApproximateMIS) k_shade<3, true, true, true, false, true, true><<<g.smCount * 3, 128, 0, s>>>(p); else k_shade<3, true, true, true, false, false, true><<<g.smCount * 3, 128, 0, s>>>(p);
@@ -128,6 +147,7 @@ template <bool AMIS>
 static void launchShadeMis(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
 {
     const int grid = g.smCount * g.shadeBlocksPerSM;
+    if (firstHitDebugView(p)) { if (p.stf.pointTextures) launchShadeDebugViewMis<AMIS, true>(p, g, s); else launchShadeDebugViewMis<AMIS, false>(p, g, s); return; }
     if (p.stf.pointTextures)
     {   // stochastic texture filtering: one kernel per guide / sample-count choice.  4 CTAs per SM although the single-sample kernels spill 12-24 bytes there: measured on an H100,
         // k_shade on the bench workload is 7.37 ms at 4 CTAs and 7.76 ms at 3 without spills.  Like the guide and analytic-light kernels, they do not follow RTXPT_SHADE_CTAS

@@ -125,8 +125,10 @@ struct LaunchParams
     // stochastic texture filtering (kernels instantiated with STF = true only; appended for the same reason): rtxpt_b200_set_texture_filtering's filter and sigma, and per bindless
     // texture a point-filtered texture object over the same mip arrays and the texture's width, height and level count
     struct { const cudaTextureObject_t* pointTextures; const uint4* textureDims; uint filterType; float sigma; } stf;
+    // debug view (rtxpt_b200_set_debug_view; read by the kernels instantiated for it only, appended for the same reason): the RGBA16F target, the view, the stable plane it shows
+    struct { uint2* viz; uint view; int planeIndex; } dbg;
 };
-static_assert(sizeof(LaunchParams) == 1656, "the parameter block of every kernel keeps its layout");
+static_assert(sizeof(LaunchParams) == 1672, "the parameter block of every kernel keeps its layout");
 
 // ---- NEE blocks (NEEFullSamples = N > 1) ---------------------------------------------------------------------------------------------------------------
 // A vertex that takes light samples appends one block of 1 + N uint4 (counter kCtrNeeBlocks) to LaunchParams::neeBlocks: a header { path slot or home index h, the FILL

@@ -51,6 +51,7 @@ _SIGNATURES = {
     "rtxpt_b200_set_view": [C.c_void_p, C.c_void_p],
     "rtxpt_b200_set_realtime": [C.c_void_p, C.POINTER(S.RealtimeConstants)],
     "rtxpt_b200_set_texture_filtering": [C.c_void_p, C.POINTER(S.StochasticTextureFiltering)],
+    "rtxpt_b200_set_debug_view": [C.c_void_p, C.POINTER(S.DebugView)],
     "rtxpt_b200_path_trace_realtime": [C.c_void_p, C.c_int, C.c_void_p],
     "rtxpt_b200_denoiser_prepare_inputs": [C.c_void_p, C.c_uint32, C.c_int, C.POINTER(S.DenoiserConstants), C.c_void_p],
     "rtxpt_b200_denoiser_final_merge": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p],
@@ -339,6 +340,18 @@ class Context:
         """Stochastic texture filtering of every material fetch (RTXPT's STFFilterMode / STFMagnificationMethod / STFGaussianSigma); raises and keeps the previous setting
         when the description is refused"""
         _check(self.L.rtxpt_b200_set_texture_filtering(self.h, C.byref(S.StochasticTextureFiltering(int(enable), filter_type, magnification_method, gaussian_sigma))), self.L)
+
+    def set_debug_view(self, view, stable_plane_index=S.DEBUG_VIEW_STABLE_PLANE_SPLIT):
+        """RTXPT's debug view (m_ui.DebugView / DebugViewStablePlaneIndex): `view` is a DebugViewType value or name (structs.DEBUG_VIEW_NAMES); raises and keeps the previous
+        view when it is refused"""
+        if isinstance(view, str): view = S.DEBUG_VIEW[view]
+        _check(self.L.rtxpt_b200_set_debug_view(self.h, C.byref(S.DebugView(view, stable_plane_index & 0xFFFFFFFF))), self.L)
+
+    def readback_debug_view(self):
+        """RTXPT_BUFFER_DEBUG_VIZ_F16 as float16 [H, W, 4]"""
+        out = np.empty((self.consts.imageHeight, self.consts.imageWidth, 4), np.float16)
+        _check(self.L.rtxpt_b200_readback(self.h, S.BUFFER_DEBUG_VIZ_F16, out.ctypes.data, out.nbytes), self.L)
+        return out
 
     def set_realtime(self, rt):
         self.realtime = rt

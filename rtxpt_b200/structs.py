@@ -40,6 +40,7 @@ STABLE_PLANE_COUNT, STABLE_PLANE_INVALID_BRANCH = 3, 0xFFFFFFFF
 BUFFER_DENOISED_DIFF_RADIANCE_HITDIST_F16, BUFFER_DENOISED_SPEC_RADIANCE_HITDIST_F16, BUFFER_REBLUR_ACCUMULATED_FRAMES_RG8 = 16, 17, 18
 BUFFER_LDR_COLOR_RGBA8 = 19
 BUFFER_STABLE_PLANE_NEIGHBOUR_GUIDES = 20        # exchange only (rtxpt_b200_exchange_*)
+BUFFER_DEBUG_VIZ_F16 = 21                        # rtxpt_b200_set_debug_view
 
 
 class GeometryData(C.Structure):
@@ -195,6 +196,41 @@ class StochasticTextureFiltering(C.Structure):
 
 
 STF_FILTER_POINT, STF_FILTER_LINEAR, STF_FILTER_CUBIC, STF_FILTER_GAUSSIAN = 0, 1, 2, 3
+
+
+class DebugView(C.Structure):
+    """RtxptDebugView (rtxpt_b200_set_debug_view): debugViewType is RTXPT's DebugViewType, stablePlaneIndex 0..2 or DEBUG_VIEW_STABLE_PLANE_SPLIT"""
+    _fields_ = [("debugViewType", u32), ("stablePlaneIndex", u32)]
+
+
+# DebugViewType (Rtxpt/Shaders/PathTracer/PathTracerDebug.hlsli:25-65), in order
+DEBUG_VIEW_NAMES = (
+    "Disabled", "DominantStablePlaneIndex",
+    "StablePlane_VirtualRayLength", "StablePlane_MotionVectors", "StablePlane_Normals", "StablePlane_Roughness", "StablePlane_SpecAvg", "StablePlane_DiffBSDFEstimate",
+    "StablePlane_DiffRadiance", "StablePlane_SpecBSDFEstimate", "StablePlane_SpecRadiance", "StablePlane_RelaxedDisocclusion", "StablePlane_DiffRadianceDenoised",
+    "StablePlane_SpecRadianceDenoised", "StablePlane_CombinedRadianceDenoised", "StablePlane_ViewZ", "StablePlane_Throughput", "StablePlane_DenoiserValidation",
+    "StableRadiance",
+    "DenoiserGuide_Depth", "DenoiserGuide_Roughness", "DenoiserGuide_Albedo", "DenoiserGuide_SpecAlbedo", "DenoiserGuide_Normal", "DenoiserGuide_MotionVectors",
+    "DenoiserGuide_SpecMotionVectors", "DenoiserGuide_SpecHitT", "DenoiserGuide_LayerWeights", "DenoiserGuide_PrimaryLayer",
+    "FirstHit_Barycentrics", "FirstHit_FaceNormal", "FirstHit_GeometryNormal", "FirstHit_ShadingNormal", "FirstHit_ShadingTangent", "FirstHit_ShadingBitangent",
+    "FirstHit_FrontFacing", "FirstHit_ThinSurface", "FirstHit_Diffuse", "FirstHit_Specular", "FirstHit_Roughness", "FirstHit_Metallic", "FirstHit_ShaderID", "FirstHit_MaterialID",
+    "VBufferMotionVectors", "VBufferDepth",
+    "SecondarySurfacePosition", "SecondarySurfaceRadiance", "ReSTIRGIOutput",
+    "ReSTIRDIInitialOutput", "ReSTIRDITemporalOutput", "ReSTIRDISpatialOutput", "ReSTIRDIFinalOutput", "ReSTIRDIFinalContribution", "ReGIRIndirectOutput",
+)
+DEBUG_VIEW = {name: i for i, name in enumerate(DEBUG_VIEW_NAMES)}
+DEBUG_VIEW_MAX_COUNT = len(DEBUG_VIEW_NAMES)
+DEBUG_VIEW_STABLE_PLANE_SPLIT = 0xFFFFFFFF
+DEBUG_VIEWS_FIRST_HIT = tuple(range(DEBUG_VIEW["FirstHit_Barycentrics"], DEBUG_VIEW["FirstHit_MaterialID"] + 1))
+DEBUG_VIEWS_STABLE_PLANES = tuple(range(DEBUG_VIEW["DominantStablePlaneIndex"], DEBUG_VIEW["StablePlane_SpecRadiance"] + 1)) + (DEBUG_VIEW["StableRadiance"],)
+DEBUG_VIEWS_DENOISER_MERGE = tuple(range(DEBUG_VIEW["StablePlane_RelaxedDisocclusion"], DEBUG_VIEW["StablePlane_DenoiserValidation"] + 1))
+
+
+def debug_view_status(view, stable_plane_index=DEBUG_VIEW_STABLE_PLANE_SPLIT):
+    """What rtxpt_b200_set_debug_view returns for a description: 0, or RTXPT_ERR_INVALID_ARGUMENT (-1) / RTXPT_ERR_UNSUPPORTED (-6)"""
+    if not 0 <= view < DEBUG_VIEW_MAX_COUNT or not (0 <= stable_plane_index < 3 or stable_plane_index == DEBUG_VIEW_STABLE_PLANE_SPLIT):
+        return -1
+    return 0 if view == DEBUG_VIEW["Disabled"] or view in DEBUG_VIEWS_FIRST_HIT + DEBUG_VIEWS_STABLE_PLANES + DEBUG_VIEWS_DENOISER_MERGE else -6
 
 
 class PathTracerConstants(C.Structure):
