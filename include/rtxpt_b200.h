@@ -611,6 +611,37 @@ enum {
     RTXPT_BUFFER_REBLUR_ACCUMULATED_FRAMES_RG8      = 18   /* NRD's DATA1 after TemporalAccumulation: accumulated frames / 63 (diffuse, specular) */
 };
 RTXPT_API int rtxpt_b200_reblur_denoise(rtxpt_ctx* ctx, uint32_t stablePlaneIndex, const RtxptReblurFrame* frame, void* cudaStream);
+/* ReBLUR settings: the nrd::ReblurSettings fields RTXPT's denoiser panel sets (Denoiser -> Advanced Settings, Rtxpt/SampleUI.cpp:1360-1410; m_ui.ReblurSettings, which Sample.cpp:2606-2610
+ * hands to NrdIntegration::RunDenoiserPasses every frame) and m_ui.NRDUseAlternateDisocclusionThresholdMix (CommonSettings::isDisocclusionThresholdMixAvailable).
+ * rtxpt_b200_default_reblur_settings gives NRD's defaults with RTXPT's overrides (NrdConfig.cpp:49-61): what a context uses until rtxpt_b200_set_reblur_settings is called.
+ * rtxpt_b200_set_reblur_settings applies from the next reblur_denoise / denoise_realtime, to every plane's instance; as in NRD, a change keeps the history.  Refused with
+ * RTXPT_ERR_INVALID_ARGUMENT, keeping the previous settings: a non-finite value, a negative radius, lobeAngleFraction / roughnessFraction / responsiveAccumulationRoughnessThreshold /
+ * planeDistanceSensitivity outside [0, 1], a frame count above 63 (REBLUR_MAX_HISTORY_FRAME_NUM), a reconstruction mode above 2, a flag above 1.
+ * hitDistanceParameters decode the normalised hit distances of the inputs.  As in RTXPT, which feeds one struct to both, the caller passes the same four values here and in
+ * RtxptDenoiserConstants::hitDistanceParameters (which normalise them in rtxpt_b200_denoiser_prepare_inputs); the library does not check that they agree.
+ * The passes follow NRD's dispatch graph (Reblur.cpp:117-160): hitDistanceReconstructionMode OFF skips HitDistReconstruction; both pre-pass radii 0 skip the PrePass. */
+typedef struct RtxptReblurSettings {
+    float hitDistanceParameters[4];                 /* HitDistanceParameters A, B, C, D (3, 0.1, 20, -25) */
+    float antilagLuminanceSigmaScale;               /* antilagSettings.luminanceSigmaScale (4) */
+    float antilagLuminanceSensitivity;              /* antilagSettings.luminanceSensitivity (3) */
+    uint32_t maxAccumulatedFrameNum;                /* 50 (RTXPT) */
+    uint32_t maxFastAccumulatedFrameNum;            /* 6 */
+    uint32_t historyFixFrameNum;                    /* 3 */
+    float diffusePrepassBlurRadius;                 /* pixels, 15 (RTXPT) */
+    float specularPrepassBlurRadius;                /* pixels, 40 (RTXPT) */
+    float minBlurRadius, maxBlurRadius;             /* pixels, 1 / 30 */
+    float lobeAngleFraction, roughnessFraction;     /* 0.15 / 0.15 */
+    float responsiveAccumulationRoughnessThreshold; /* 0 */
+    float planeDistanceSensitivity;                 /* 0.02 */
+    uint32_t hitDistanceReconstructionMode;         /* RTXPT_REBLUR_HIT_DISTANCE_RECONSTRUCTION_* (AREA_5X5, RTXPT) */
+    uint32_t enableAntiFirefly;                     /* 1 (RTXPT) */
+    uint32_t useAlternateDisocclusionThresholdMix;  /* 1 (SampleUI.h:295): blend towards disocclusionThresholdAlternate by RTXPT_BUFFER_DENOISER_DISOCCLUSION_MIX_R8 */
+} RtxptReblurSettings;
+#define RTXPT_REBLUR_HIT_DISTANCE_RECONSTRUCTION_OFF        0u
+#define RTXPT_REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_3X3   1u
+#define RTXPT_REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_5X5   2u
+RTXPT_API int rtxpt_b200_default_reblur_settings(RtxptReblurSettings* out);
+RTXPT_API int rtxpt_b200_set_reblur_settings(rtxpt_ctx* ctx, const RtxptReblurSettings* settings);
 /* Sample::Denoise for the ReBLUR method (Rtxpt/Sample.cpp:2560-2618): for plane = active-1 .. 0 { prepare_inputs (first: init with stable radiance); reblur_denoise; final_merge } */
 RTXPT_API int rtxpt_b200_denoise_realtime(rtxpt_ctx* ctx, const RtxptDenoiserConstants* constants, const RtxptReblurFrame* frame, void* cudaStream);
 /* device time (CUDA events on the call's stream) of the last rtxpt_b200_denoise_realtime; waits for it to finish */

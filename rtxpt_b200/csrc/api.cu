@@ -169,6 +169,7 @@ struct rtxpt_ctx
         DeviceArray<float> prevViewZ; DeviceArray<uint32_t> prevNormalRoughness; DeviceArray<uint16_t> prevInternalData, diffFast, specFast, tracking[2], diffLuma[2], specLuma[2];
         DeviceArray<uint2> diffHistory, specHistory; bool valid = false; uint32_t pingPong = 0;
     } reblur[RTXPT_STABLE_PLANE_COUNT];
+    RtxptReblurSettings reblurSettings = rb::defaultSettings();                                 // rtxpt_b200_set_reblur_settings; every plane's instance denoises with them
     DeviceArray<uint8_t> rbTiles; DeviceArray<uint2> rbTmp1Diff, rbTmp1Spec, rbTmp2Diff, rbTmp2Spec, rbOutDiff, rbOutSpec; DeviceArray<uint16_t> rbTrackingT, rbDiffFastT, rbSpecFastT; DeviceArray<uchar2> rbData1; DeviceArray<uint32_t> rbData2;
     uint32_t reblurWidth = 0, reblurHeight = 0;
     // NEE-AT temporal feedback (consts.NEEType == 2 && consts.NEEATFeedback): LightsBaker's frame state, reservoirs, tile samplers and the per-frame global proxy table
@@ -1597,9 +1598,11 @@ extern "C" RTXPT_API int rtxpt_b200_reblur_denoise(rtxpt_ctx* c, uint32_t stable
     int rc = ensureReblurPools(c, s); if (rc != RTXPT_OK) return rc;
     rtxpt_ctx::ReblurHistory& h = c->reblur[stablePlaneIndex];
     const uint32_t W = c->tableWidth, H = c->tableHeight;
-    rb::Params p{}; rb::fillFrameParams(p, W, H, f, h.valid);
-    // resources
-    p.viewZ = c->dnViewZ.ptr; p.normalRoughness = c->dnNormalRoughness.ptr; p.motion = f->ignoreMotionVectors ? nullptr : c->dnMotion.ptr; p.disocclusionMix = c->dnDisocclusionMix.ptr; p.inDiff = c->dnDiff.ptr; p.inSpec = c->dnSpec.ptr;
+    const RtxptReblurSettings& settings = c->reblurSettings;
+    rb::Params p{}; rb::fillFrameParams(p, W, H, f, h.valid, settings);
+    // resources; without the disocclusion-threshold mix (isDisocclusionThresholdMixAvailable false) TemporalAccumulation reads a mix of 0
+    p.viewZ = c->dnViewZ.ptr; p.normalRoughness = c->dnNormalRoughness.ptr; p.motion = f->ignoreMotionVectors ? nullptr : c->dnMotion.ptr;
+    p.disocclusionMix = settings.useAlternateDisocclusionThresholdMix ? c->dnDisocclusionMix.ptr : nullptr; p.inDiff = c->dnDiff.ptr; p.inSpec = c->dnSpec.ptr;
     p.tiles = c->rbTiles.ptr; p.tmp1Diff = c->rbTmp1Diff.ptr; p.tmp1Spec = c->rbTmp1Spec.ptr; p.tmp2Diff = c->rbTmp2Diff.ptr; p.tmp2Spec = c->rbTmp2Spec.ptr;
     p.trackingTransient = c->rbTrackingT.ptr; p.diffFastTransient = c->rbDiffFastT.ptr; p.specFastTransient = c->rbSpecFastT.ptr; p.data1 = c->rbData1.ptr; p.data2 = c->rbData2.ptr;
     p.prevViewZ = h.prevViewZ.ptr; p.prevNormalRoughness = h.prevNormalRoughness.ptr; p.prevInternalData = h.prevInternalData.ptr; p.diffHistory = h.diffHistory.ptr; p.specHistory = h.specHistory.ptr;
@@ -1607,9 +1610,24 @@ extern "C" RTXPT_API int rtxpt_b200_reblur_denoise(rtxpt_ctx* c, uint32_t stable
     const uint32_t prev = h.pingPong, curr = prev ^ 1u;
     p.trackingPrev = h.tracking[prev].ptr; p.trackingCurr = h.tracking[curr].ptr; p.diffLumaPrev = h.diffLuma[prev].ptr; p.diffLumaCurr = h.diffLuma[curr].ptr; p.specLumaPrev = h.specLuma[prev].ptr; p.specLumaCurr = h.specLuma[curr].ptr;
     p.outDiff = c->rbOutDiff.ptr; p.outSpec = c->rbOutSpec.ptr;
-    launchReblurFrame(p, !(c->cfg.flags & RTXPT_CFG_REBLUR_UNTILED), s);
+    launchReblurFrame(p, settings.hitDistanceReconstructionMode, !(c->cfg.flags & RTXPT_CFG_REBLUR_UNTILED), s);
     CU(cudaGetLastError());
     h.pingPong = curr; h.valid = true;
+    return RTXPT_OK;
+}
+
+extern "C" RTXPT_API int rtxpt_b200_default_reblur_settings(RtxptReblurSettings* out)
+{
+    if (!out) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    *out = rb::defaultSettings();
+    return RTXPT_OK;
+}
+// m_ui.ReblurSettings -> nrd::SetDenoiserSettings (NrdIntegration.cpp:364-368): taken from the next frame on, history kept
+extern "C" RTXPT_API int rtxpt_b200_set_reblur_settings(rtxpt_ctx* c, const RtxptReblurSettings* settings)
+{
+    if (!c || !settings) return fail(RTXPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (const char* why = rb::settingsError(*settings)) return fail(RTXPT_ERR_INVALID_ARGUMENT, "ReBLUR settings refused: %s", why);
+    c->reblurSettings = *settings;
     return RTXPT_OK;
 }
 

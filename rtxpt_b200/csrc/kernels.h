@@ -61,6 +61,7 @@ namespace neeat { struct Params; }
 void launchNeeatUpdateBegin(const neeat::Params& p, bool preFilter, uint* scanBlockSums, int smCount, cudaStream_t s);     // neeat_kernels.cu
 void launchNeeatUpdateEnd(const neeat::Params& p, cudaStream_t s);
 namespace rb { struct Params; }
-void launchReblurFrame(const rb::Params& p, bool tiled, cudaStream_t s);       // reblur_kernels.cu: the eight ReBLUR passes of one stable plane; tiled: HitDistReconstruction through shared memory
+// reblur_kernels.cu: the ReBLUR passes of one stable plane that the settings select (rb::routeFrame: hit-distance reconstruction mode, pre-pass radii in p); tiled: HitDistReconstruction through shared memory
+void launchReblurFrame(const rb::Params& p, uint32_t hitDistanceReconstructionMode, bool tiled, cudaStream_t s);
 
 } // namespace pt

@@ -1,6 +1,6 @@
-// reblur_host.h - host half of the ReBLUR denoiser: nrd::ReblurSettings as RTXPT sets them (Rtxpt/NRD/NrdConfig.cpp:49-61), nrd::CommonSettings (NrdIntegration.cpp:375-408) and the
+// reblur_host.h - host half of the ReBLUR denoiser: nrd::ReblurSettings (RTXPT's defaults: Rtxpt/NRD/NrdConfig.cpp:49-61; the fields its panel sets: RtxptReblurSettings), nrd::CommonSettings (NrdIntegration.cpp:375-408) and the
 // per-frame constants NRD derives from the matrices (External/Nrd/Source/InstanceImpl.cpp:331-451, Reblur.cpp:280-392): camera-relative matrices, frustum, unproject, kernel
-// rotators.  Plain C++ on top of rb::Params; used by api.cu and by the test-only host build of the passes (tests/emu/reblur_host_emu.cu).
+// rotators, and the pass routing the settings select.  Plain C++ on top of rb::Params; used by api.cu, reblur_kernels.cu and by the test-only host builds of the passes (tests/emu/reblur_host_emu.cu, reblur_settings_host_emu.cu).
 #pragma once
 #include "reblur.cuh"
 #include "../../include/rtxpt_b200.h"
@@ -26,8 +26,36 @@ inline void rbRelativeWorldToClip(const float* wv, const float* camRel, const fl
 }
 
 
-// everything of rb::Params except the resource pointers; historyValid = this plane's instance has denoised a frame since its creation / last resize
-inline void fillFrameParams(Params& p, uint32_t W, uint32_t H, const RtxptReblurFrame* f, bool historyValid)
+// nrd::ReblurSettings defaults (NRDSettings.h:230-300) with RTXPT's overrides (Rtxpt/NRD/NrdConfig.cpp:49-61): enableAntiFirefly, AREA_5X5, maxAccumulatedFrameNum 50, pre-pass radii 15 / 40
+inline RtxptReblurSettings defaultSettings()
+{
+    RtxptReblurSettings s;
+    s.hitDistanceParameters[0] = 3.0f; s.hitDistanceParameters[1] = 0.1f; s.hitDistanceParameters[2] = 20.0f; s.hitDistanceParameters[3] = -25.0f;
+    s.antilagLuminanceSigmaScale = 4.0f; s.antilagLuminanceSensitivity = 3.0f;
+    s.maxAccumulatedFrameNum = 50; s.maxFastAccumulatedFrameNum = 6; s.historyFixFrameNum = 3;
+    s.diffusePrepassBlurRadius = 15.0f; s.specularPrepassBlurRadius = 40.0f; s.minBlurRadius = 1.0f; s.maxBlurRadius = 30.0f;
+    s.lobeAngleFraction = 0.15f; s.roughnessFraction = 0.15f; s.responsiveAccumulationRoughnessThreshold = 0.0f; s.planeDistanceSensitivity = 0.02f;
+    s.hitDistanceReconstructionMode = RTXPT_REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_5X5; s.enableAntiFirefly = 1; s.useAlternateDisocclusionThresholdMix = 1;
+    return s;
+}
+// what rtxpt_b200_set_reblur_settings refuses: NULL when `s` is accepted, else the reason
+inline const char* settingsError(const RtxptReblurSettings& s)
+{
+    const float all[] = { s.hitDistanceParameters[0], s.hitDistanceParameters[1], s.hitDistanceParameters[2], s.hitDistanceParameters[3], s.antilagLuminanceSigmaScale, s.antilagLuminanceSensitivity,
+                          s.diffusePrepassBlurRadius, s.specularPrepassBlurRadius, s.minBlurRadius, s.maxBlurRadius, s.lobeAngleFraction, s.roughnessFraction,
+                          s.responsiveAccumulationRoughnessThreshold, s.planeDistanceSensitivity };
+    for (float v : all) if (!std::isfinite(v)) return "every value must be finite";
+    if (s.diffusePrepassBlurRadius < 0.0f || s.specularPrepassBlurRadius < 0.0f || s.minBlurRadius < 0.0f || s.maxBlurRadius < 0.0f) return "radii must not be negative";
+    const float fractions[] = { s.lobeAngleFraction, s.roughnessFraction, s.responsiveAccumulationRoughnessThreshold, s.planeDistanceSensitivity };
+    for (float v : fractions) if (v < 0.0f || v > 1.0f) return "lobeAngleFraction, roughnessFraction, responsiveAccumulationRoughnessThreshold and planeDistanceSensitivity lie in [0, 1]";
+    if (s.maxAccumulatedFrameNum > 63 || s.maxFastAccumulatedFrameNum > 63 || s.historyFixFrameNum > 63) return "frame counts lie in [0, 63] (REBLUR_MAX_HISTORY_FRAME_NUM)";
+    if (s.hitDistanceReconstructionMode > RTXPT_REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_5X5) return "hitDistanceReconstructionMode: OFF (0), AREA_3X3 (1) or AREA_5X5 (2)";
+    if (s.enableAntiFirefly > 1 || s.useAlternateDisocclusionThresholdMix > 1) return "enableAntiFirefly and useAlternateDisocclusionThresholdMix are 0 or 1";
+    return nullptr;
+}
+
+// everything of rb::Params except the resource pointers, for settings `s`; historyValid = this plane's instance has denoised a frame since its creation / last resize
+inline void fillFrameParams(Params& p, uint32_t W, uint32_t H, const RtxptReblurFrame* f, bool historyValid, const RtxptReblurSettings& s = defaultSettings())
 {
     p.W = W; p.H = H; p.tilesW = (W + 15) / 16; p.frameIndex = f->frameIndex;
     for (int r = 0; r < 3; r++) for (int k = 0; k < 3; k++) p.viewToWorld[r * 3 + k] = f->matWorldToView[k * 4 + r];
@@ -43,19 +71,44 @@ inline void fillFrameParams(Params& p, uint32_t W, uint32_t H, const RtxptReblur
     p.rotatorPre = rbRotator(rbWeyl(0.5f, f->frameIndex) * rad90);
     p.rotator = rbCombine(rbRotator(rbWeyl(0.0f, f->frameIndex * 2) * rad90), rbRotator(float((f->frameIndex * 2) & 15u) / 16.0f * rad360));
     p.rotatorPost = rbCombine(rbRotator(rbWeyl(0.0f, f->frameIndex * 2 + 1) * rad90), rbRotator(float((f->frameIndex * 2 + 1) & 15u) / 16.0f * rad360));
-    // settings: RTXPT's ReBLUR configuration
+    // settings (AddSharedConstants_Reblur, Reblur.cpp:284-388); the rest are NRD's defaults, which RTXPT's panel does not expose
     const bool reset = f->resetHistory != 0 || !historyValid;
-    const float hitDist[4] = { 3.0f, 0.1f, 20.0f, -25.0f }; memcpy(p.hitDistParams, hitDist, 16);
-    p.maxAccumulatedFrameNum = reset ? 0.0f : 50.0f; p.maxFastAccumulatedFrameNum = reset ? 0.0f : 6.0f; p.historyFixFrameNum = 3.0f; p.historyFixBasePixelStride = 14.0f;
-    p.diffPrepassBlurRadius = 15.0f; p.specPrepassBlurRadius = 40.0f; p.minBlurRadius = 1.0f; p.maxBlurRadius = 30.0f; p.lobeAngleFraction = 0.15f * 0.15f; p.roughnessFraction = 0.15f;
-    p.planeDistSensitivity = 0.02f; p.minHitDistanceWeight = 0.1f; p.minMaterialDiff = 4.0f; p.minMaterialSpec = 4.0f; p.denoisingRange = 100000.0f; p.viewZScale = 1.0f;
+    memcpy(p.hitDistParams, s.hitDistanceParameters, 16);
+    p.maxAccumulatedFrameNum = reset ? 0.0f : float(std::min(s.maxAccumulatedFrameNum, 63u)); p.maxFastAccumulatedFrameNum = reset ? 0.0f : float(s.maxFastAccumulatedFrameNum);
+    p.historyFixFrameNum = float(s.historyFixFrameNum); p.historyFixBasePixelStride = 14.0f;
+    p.diffPrepassBlurRadius = s.diffusePrepassBlurRadius; p.specPrepassBlurRadius = s.specularPrepassBlurRadius; p.minBlurRadius = s.minBlurRadius; p.maxBlurRadius = std::max(s.maxBlurRadius, s.minBlurRadius);
+    p.lobeAngleFraction = s.lobeAngleFraction * s.lobeAngleFraction; p.roughnessFraction = s.roughnessFraction;
+    p.planeDistSensitivity = s.planeDistanceSensitivity; p.minHitDistanceWeight = 0.1f; p.minMaterialDiff = 4.0f; p.minMaterialSpec = 4.0f; p.denoisingRange = 100000.0f; p.viewZScale = 1.0f;
     const float thresholdBonus = 1.0f / float(H);           // ( 1 + jitterDelta ) / rectH, Reblur.cpp:293; un-jittered matrices
     p.disocclusionThreshold = (f->disocclusionThreshold > 0.0f ? f->disocclusionThreshold : 0.03f) + thresholdBonus;
     p.disocclusionThresholdAlternate = (f->disocclusionThresholdAlternate > 0.0f ? f->disocclusionThresholdAlternate : 0.2f) + thresholdBonus;
     p.framerateScale = f->frameTimeMs > 0.0f ? std::max(33.333f / f->frameTimeMs, 1.0f) : 2.0f;          // max( 33.333 ms / frame time, 1 ), Reblur.cpp:296
-    p.fireflySuppressorMinRelativeScale = 2.0f; p.responsiveAccumulationRoughnessThreshold = 0.0f;
-    p.antilagSigmaScale = 4.0f; p.antilagSensitivity = 3.0f; p.stabilizationStrength = reset ? 0.0f : 63.0f / 64.0f;
-    p.antiFirefly = 1; p.usePrepassOnlyForSpecularMotionEstimation = 0;
+    p.fireflySuppressorMinRelativeScale = 2.0f; p.responsiveAccumulationRoughnessThreshold = s.responsiveAccumulationRoughnessThreshold;
+    p.antilagSigmaScale = s.antilagLuminanceSigmaScale; p.antilagSensitivity = s.antilagLuminanceSensitivity; p.stabilizationStrength = reset ? 0.0f : 63.0f / 64.0f;
+    p.antiFirefly = s.enableAntiFirefly; p.usePrepassOnlyForSpecularMotionEstimation = 0;
+}
+
+// NRD's dispatch graph for the settings (Reblur.cpp:117-160, Reblur_DiffuseSpecular.hpp:83-169): which of HitDistReconstruction and PrePass run, and the Params each pass of
+// the three at the head of the chain is launched with.  The pass bodies read and write fixed fields (reconstruction: in -> tmp2, PrePass: tmp2 -> tmp1, TemporalAccumulation:
+// tmp1 -> tmp2); the routing points those fields at the images NRD binds for the permutation:
+//   HitDistReconstruction   -> TEMP2 ahead of a PrePass, else -> TEMP1
+//   PrePass                 TEMP2 after a reconstruction, else IN ->
+//   TemporalAccumulation    TEMP1 after either of them, else IN
+// clearSpecTmp1: TemporalAccumulation reads the hit distance of its 3x3 neighbourhood from its specular input when specularPrepassBlurRadius is 0 (REBLUR_TemporalAccumulation.hlsli:32);
+// when that input is TEMP1, the pixels the writing pass skips (sky tiles, beyond the denoising range) would hold whatever an earlier pass left there, which NRD leaves undefined.
+// TEMP1 is cleared first, so that they read as "no hit distance".
+struct FrameRouting { int reconstructionRadius; bool prePass, clearSpecTmp1; Params reconstruction, pre, temporal; };
+inline FrameRouting routeFrame(const Params& p, uint32_t hitDistanceReconstructionMode)
+{
+    FrameRouting r;
+    r.reconstructionRadius = hitDistanceReconstructionMode == RTXPT_REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_5X5 ? 2 : (hitDistanceReconstructionMode == RTXPT_REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_3X3 ? 1 : 0);
+    r.prePass = p.diffPrepassBlurRadius != 0.0f || p.specPrepassBlurRadius != 0.0f;
+    r.clearSpecTmp1 = p.specPrepassBlurRadius == 0.0f && (r.reconstructionRadius != 0 || r.prePass);
+    r.reconstruction = p; r.pre = p; r.temporal = p;
+    if (!r.prePass) { r.reconstruction.tmp2Diff = p.tmp1Diff; r.reconstruction.tmp2Spec = p.tmp1Spec; }
+    if (r.reconstructionRadius == 0) { r.pre.tmp2Diff = const_cast<uint2*>(p.inDiff); r.pre.tmp2Spec = const_cast<uint2*>(p.inSpec); }
+    if (r.reconstructionRadius == 0 && !r.prePass) { r.temporal.tmp1Diff = const_cast<uint2*>(p.inDiff); r.temporal.tmp1Spec = const_cast<uint2*>(p.inSpec); }
+    return r;
 }
 
 } } // namespace pt::rb

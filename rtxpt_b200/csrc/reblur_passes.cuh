@@ -3,7 +3,7 @@
 // NRD's REBLUR_DIFFUSE_SPECULAR chain for one stable plane (SURVEY §8 row a18 / K9), pass by pass along the dispatch graph
 // (External/Nrd/Source/Denoisers/Reblur_DiffuseSpecular.hpp:71-270) in RTXPT's configuration (Rtxpt/NRD/NrdConfig.cpp:49-61, NrdIntegration.cpp:375-408):
 //   beyondDenoisingRange            REBLUR_ClassifyTiles.cs.hlsl:21-60 (the per-texel predicate; the kernel counts it over a 16x16 tile)
-//   hitDistReconstructionPixel      REBLUR_HitDistReconstruction.hlsli:11-155 (5x5)
+//   hitDistReconstructionPixel      REBLUR_HitDistReconstruction.hlsli:11-155 (5x5 or 3x3)
 //   spatialPixel<PRE|BLUR|POST>     REBLUR_PrePass / REBLUR_Blur / REBLUR_PostBlur.hlsli + REBLUR_Common_{Diffuse,Specular}SpatialFilter.hlsli
 //   temporalAccumulationPixel       REBLUR_TemporalAccumulation.hlsli:11-937
 //   historyFixPixel                 REBLUR_HistoryFix.hlsli:11-496
@@ -41,7 +41,7 @@ PT_HD bool beyondDenoisingRange(const Params& p, int x, int y)
     return z > p.denoisingRange;
 }
 
-// ---- HitDistReconstruction 5x5: in -> tmp2 ------------------------------------------------------------------------------------------------------------------------
+// ---- HitDistReconstruction 5x5 / 3x3: in -> tmp2 (which images those are: routeFrame, reblur_host.h) ------------------------------------------------------------------------------------------------------------------------
 // The 5x5 neighbourhood comes through a tap source: straight from global memory (GlobalTaps: the host build and the border tiles' fallback) or from the CTA's shared-memory
 // tile (reblur_kernels.cu: viewZ, the UNPACKED normal / roughness and the two hit distances of the 20x20 region staged by TMA) - what NRD's PRELOAD_INTO_SMEM does for the same
 // pass (External/Nrd/Shaders/Include/Common.hlsli:143-175): the saving is the 24 normal unpacks and clamped address computations per pixel, not bandwidth.
@@ -53,7 +53,8 @@ struct GlobalTaps
     PT_HD float diffHitDist(int qx, int qy) const { return f16tof32(p.inDiff[size_t(qy) * W + qx].y >> 16); }
     PT_HD float specHitDist(int qx, int qy) const { return f16tof32(p.inSpec[size_t(qy) * W + qx].y >> 16); }
 };
-template <typename Taps>
+// RADIUS 2: REBLUR_DiffuseSpecular_HitDistReconstruction_5x5.cs.hlsl (NRD_USE_BORDER_2); RADIUS 1: REBLUR_DiffuseSpecular_HitDistReconstruction.cs.hlsl (AREA_3X3, BORDER 1) - the same body
+template <int RADIUS, typename Taps>
 PT_HD void hitDistReconstructionBody(const Params& p, const int x, const int y, const Taps& taps)
 {
     RB_PIXEL_PROLOGUE;
@@ -65,7 +66,7 @@ PT_HD void hitDistReconstructionBody(const Params& p, const int x, const int y, 
     const float4 d = unpackRGBA16F(p.inDiff[pix]), s = unpackRGBA16F(p.inSpec[pix]);
     float cx = d.w, cy = s.w, sx = cx != 0.0f ? 1000.0f : 0.0f, sy = cy != 0.0f ? 1000.0f : 0.0f;
     cx *= sx; cy *= sy;
-    for (int j = -2; j <= 2; j++) for (int i = -2; i <= 2; i++)
+    for (int j = -RADIUS; j <= RADIUS; j++) for (int i = -RADIUS; i <= RADIUS; i++)
     {
         if (i == 0 && j == 0) continue;
         const int qx = clampi(x + i, 0, W - 1), qy = clampi(y + j, 0, H - 1);
@@ -84,7 +85,8 @@ PT_HD void hitDistReconstructionBody(const Params& p, const int x, const int y, 
     cx /= fmaxf(sx, kEps); cy /= fmaxf(sy, kEps);
     p.tmp2Diff[pix] = packRGBA16F(make_float4(d.x, d.y, d.z, cx)); p.tmp2Spec[pix] = packRGBA16F(make_float4(s.x, s.y, s.z, cy));
 }
-PT_HD void hitDistReconstructionPixel(const Params& p, const int x, const int y) { const GlobalTaps t{ p, int(p.W), int(p.H) }; hitDistReconstructionBody(p, x, y, t); }
+template <int RADIUS = 2>
+PT_HD void hitDistReconstructionPixel(const Params& p, const int x, const int y) { const GlobalTaps t{ p, int(p.W), int(p.H) }; hitDistReconstructionBody<RADIUS>(p, x, y, t); }
 
 // ---- spatial passes ----------------------------------------------------------------------------------------------------------------------------------------------------
 // MODE 0 PrePass: tmp2 -> tmp1 (+ hit distance for tracking); 1 Blur: tmp1 -> tmp2 (+ viewZ copy into the history); 2 PostBlur: tmp2 -> history (+ normal/roughness copy)

@@ -77,6 +77,8 @@ _SIGNATURES = {
     "rtxpt_b200_reblur_denoise": [C.c_void_p, C.c_uint32, C.POINTER(S.ReblurFrame), C.c_void_p],
     "rtxpt_b200_denoise_realtime": [C.c_void_p, C.POINTER(S.DenoiserConstants), C.POINTER(S.ReblurFrame), C.c_void_p],
     "rtxpt_b200_last_denoise_ms": [C.c_void_p, C.POINTER(C.c_float)],
+    "rtxpt_b200_default_reblur_settings": [C.POINTER(S.ReblurSettings)],
+    "rtxpt_b200_set_reblur_settings": [C.c_void_p, C.POINTER(S.ReblurSettings)],
     "rtxpt_b200_get_lights_ex": [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)],
     "rtxpt_b200_debug_bsdf": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p],
     "rtxpt_b200_debug_rng": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p],
@@ -495,6 +497,11 @@ class Context:
     # ---- ReBLUR ----
     def reblur_denoise(self, plane, frame, stream=None):
         _check(self.L.rtxpt_b200_reblur_denoise(self.h, plane, C.byref(frame), stream), self.L)
+
+    def set_reblur_settings(self, settings):
+        """RTXPT's m_ui.ReblurSettings (structs.ReblurSettings) for every plane's ReBLUR instance from the next frame on; the history stays.  Raises and keeps the previous
+        settings when they are refused (structs.reblur_settings_status says which are)."""
+        _check(self.L.rtxpt_b200_set_reblur_settings(self.h, C.byref(settings)), self.L)
 
     def denoise_realtime(self, k, frame, stream=None):
         """Sample::Denoise: for plane = active-1..0 { prepare inputs; ReBLUR; final merge } into the output colour."""

@@ -54,9 +54,11 @@ class DistGroup:
         return self.world * n
 
 
-def realtime_frame(group, denoiser_constants, reblur_frame, tone_mapping=None, feedback=False, planes=3):
-    """One frame of Sample::Render in realtime mode on `group`'s ranks (constants, view and realtime constants already set on every context).  Returns the bytes all-gathered."""
+def realtime_frame(group, denoiser_constants, reblur_frame, tone_mapping=None, feedback=False, planes=3, reblur_settings=None):
+    """One frame of Sample::Render in realtime mode on `group`'s ranks (constants, view and realtime constants already set on every context).  Returns the bytes all-gathered.
+    reblur_settings (structs.ReblurSettings, RTXPT's m_ui.ReblurSettings): applied on every rank before this frame, so that their histories stay identical."""
     stream = getattr(group, "stream", None); moved = 0
+    if reblur_settings is not None: group.each(lambda c: c.set_reblur_settings(reblur_settings))
     if feedback: group.each(lambda c: c.neeat_update_begin(stream))
     group.each(lambda c: c.path_trace_realtime(False, stream))
     moved += group.exchange(GUIDES)

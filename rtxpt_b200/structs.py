@@ -3,6 +3,7 @@ GeometryData / InstanceData (External/Donut/include/donut/shaders/bindless.h:28-
 (Rtxpt/Shaders/SubInstanceData.h:23-46), PTMaterialData (Rtxpt/Shaders/PathTracer/Materials/MaterialPT.h:45-80),
 PathTracerCameraData / PathTracerConstants (Rtxpt/Shaders/PathTracer/PathTracerShared.h:24-104)."""
 import ctypes as C
+import math
 
 u32, i32, f32, u64 = C.c_uint32, C.c_int32, C.c_float, C.c_uint64
 MAX_MIPS = 16
@@ -172,6 +173,47 @@ class ReblurFrame(C.Structure):
     _fields_ = [("matWorldToView", f32 * 16), ("matViewToClip", f32 * 16), ("prevMatWorldToView", f32 * 16), ("prevMatViewToClip", f32 * 16),
                 ("frameIndex", u32), ("resetHistory", u32), ("ignoreMotionVectors", u32), ("frameTimeMs", f32),
                 ("disocclusionThreshold", f32), ("disocclusionThresholdAlternate", f32), ("_pad", f32 * 2)]
+
+
+class ReblurSettings(C.Structure):
+    """RtxptReblurSettings (rtxpt_b200_set_reblur_settings): the nrd::ReblurSettings fields RTXPT's denoiser panel sets.  ReblurSettings.default() gives what a context uses
+    until the setter is called (NRD's defaults with RTXPT's overrides)."""
+    _fields_ = [("hitDistanceParameters", f32 * 4), ("antilagLuminanceSigmaScale", f32), ("antilagLuminanceSensitivity", f32),
+                ("maxAccumulatedFrameNum", u32), ("maxFastAccumulatedFrameNum", u32), ("historyFixFrameNum", u32),
+                ("diffusePrepassBlurRadius", f32), ("specularPrepassBlurRadius", f32), ("minBlurRadius", f32), ("maxBlurRadius", f32),
+                ("lobeAngleFraction", f32), ("roughnessFraction", f32), ("responsiveAccumulationRoughnessThreshold", f32), ("planeDistanceSensitivity", f32),
+                ("hitDistanceReconstructionMode", u32), ("enableAntiFirefly", u32), ("useAlternateDisocclusionThresholdMix", u32)]
+
+    @classmethod
+    def default(cls, **changes):
+        """RTXPT's settings (rtxpt_b200_default_reblur_settings), with `changes` (field name = value) applied"""
+        s = cls((f32 * 4)(3.0, 0.1, 20.0, -25.0), 4.0, 3.0, 50, 6, 3, 15.0, 40.0, 1.0, 30.0, 0.15, 0.15, 0.0, 0.02, REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_5X5, 1, 1)
+        for k, v in changes.items():
+            if k == "hitDistanceParameters": s.hitDistanceParameters = (f32 * 4)(*v)
+            else: setattr(s, k, v)
+        return s
+
+
+REBLUR_HIT_DISTANCE_RECONSTRUCTION_OFF, REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_3X3, REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_5X5 = 0, 1, 2
+REBLUR_MAX_HISTORY_FRAME_NUM = 63
+
+
+def reblur_settings_status(s):
+    """What rtxpt_b200_set_reblur_settings returns for `s`: 0, or RTXPT_ERR_INVALID_ARGUMENT (-1)"""
+    # ctypes hands back the stored float32 values, so the comparisons below are the library's
+    values = list(s.hitDistanceParameters) + [getattr(s, k) for k in ("antilagLuminanceSigmaScale", "antilagLuminanceSensitivity", "diffusePrepassBlurRadius",
+              "specularPrepassBlurRadius", "minBlurRadius", "maxBlurRadius", "lobeAngleFraction", "roughnessFraction", "responsiveAccumulationRoughnessThreshold", "planeDistanceSensitivity")]
+    if not all(math.isfinite(v) for v in values):
+        return -1
+    if min(s.diffusePrepassBlurRadius, s.specularPrepassBlurRadius, s.minBlurRadius, s.maxBlurRadius) < 0:
+        return -1
+    if not all(0 <= getattr(s, k) <= 1 for k in ("lobeAngleFraction", "roughnessFraction", "responsiveAccumulationRoughnessThreshold", "planeDistanceSensitivity")):
+        return -1
+    if max(s.maxAccumulatedFrameNum, s.maxFastAccumulatedFrameNum, s.historyFixFrameNum) > REBLUR_MAX_HISTORY_FRAME_NUM:
+        return -1
+    if s.hitDistanceReconstructionMode > REBLUR_HIT_DISTANCE_RECONSTRUCTION_AREA_5X5 or s.enableAntiFirefly > 1 or s.useAlternateDisocclusionThresholdMix > 1:
+        return -1
+    return 0
 
 
 class RealtimeConstants(C.Structure):
