@@ -485,6 +485,24 @@ enum {
 RTXPT_API int rtxpt_b200_denoise_spec_hit_t(rtxpt_ctx* ctx, void* cudaStream);
 RTXPT_API int rtxpt_b200_denoiser_prepare_inputs(rtxpt_ctx* ctx, uint32_t stablePlaneIndex, int initWithStableRadiance, const RtxptDenoiserConstants* constants, void* cudaStream);
 RTXPT_API int rtxpt_b200_denoiser_final_merge(rtxpt_ctx* ctx, uint32_t stablePlaneIndex, const void* dDenoisedDiffRGBA16F, const void* dDenoisedSpecRGBA16F, void* cudaStream);    /* NULL, NULL = the images rtxpt_b200_reblur_denoise wrote */
+/* ---- DLSS Ray Reconstruction's inputs (RTXPT's default realtime frame, RealtimeAA = 3): PostProcess DLSSRRDenoiserPrepareInputs, the DENOISER_DLSS_RR branch of
+ * ProcessingPasses/PostProcess.hlsl:175-440 (Sample.cpp:2710-2757).  DLSS itself (Streamline / NGX) is the host's.  Run after rtxpt_b200_path_trace_realtime(ctx, 0, s) and
+ * rtxpt_b200_denoise_spec_hit_t; per pixel it mixes the stable planes' guides by plane weights (throughput 0.2, equalisation 0.01, dominant plane +0.05), and writes
+ *   RTXPT_BUFFER_OUTPUT_COLOR_F16      (stable radiance + noisy radiance of every plane that hit a surface, scaled so that its largest channel is at most brightnessClampK, 1)
+ *   RTXPT_BUFFER_RR_*                  diffuse albedo (with the stable radiance's grey mix and a 0.05 floor), specular albedo, unit normal + roughness, and specular motion
+ *                                      vectors: plane 0's reflection hit mirrored behind a planar reflector where specular hit distance > 1e-3 and mixed roughness < 0.25,
+ *                                      RTXPT_BUFFER_MOTION_VECTORS_F16's xy elsewhere.
+ * brightnessClampK: PathTracerConstants::DLSSRRBrightnessClampK, the value the shader compares against, as Sample.cpp:1526 computes it: the UI's DLSSRRBrightnessClampK
+ * (SampleUI.h:218, default 4096) times PathTracerConstants::preExposedGrayLuminance - 4096 only without tone mapping (preExposedGrayLuminance 1, Sample.cpp:1516).  Finite and
+ * positive: RTXPT turns a UI value <= 0 into 0, which blacks the colour out, and this call refuses it.  RTXPT_ERR_INVALID_ARGUMENT before the first realtime frame at the current image
+ * size.  The four RR targets are allocated by the first call (and again after a resize); before it, readback / device_ptr refuse them. */
+RTXPT_API int rtxpt_b200_dlss_rr_prepare_inputs(rtxpt_ctx* ctx, float brightnessClampK, void* cudaStream);
+enum {
+    RTXPT_BUFFER_RR_DIFFUSE_ALBEDO_R11G11B10      = 22,   /* RRDiffuseAlbedo (RenderTargets.cpp:185-197) */
+    RTXPT_BUFFER_RR_SPECULAR_ALBEDO_R11G11B10     = 23,   /* RRSpecAlbedo */
+    RTXPT_BUFFER_RR_NORMALS_ROUGHNESS_F16         = 24,   /* RRNormalsAndRoughness RGBA16F: world-space normal, linear roughness */
+    RTXPT_BUFFER_RR_SPECULAR_MOTION_VECTORS_F16   = 25    /* RRSpecMotionVectors RG16F, pixels, current -> previous frame */
+};
 
 /* ---- Tone mapping / auto exposure (SURVEY §8f row 4; replaces ToneMappingPass::Render, Rtxpt/ToneMapper/ToneMappingPasses.cpp:230-360): log-luminance mean of the frame (auto exposure),
  * exposure, white balance / exposure-compensation colour transform, operator, clamp, sRGB encode into RTXPT_BUFFER_LDR_COLOR_RGBA8 (RTXPT's LdrColor, SRGBA8).  Field meanings and
@@ -704,6 +722,9 @@ RTXPT_API int rtxpt_b200_unpack_all(rtxpt_ctx* ctx, const void* dSrcAll, void* c
  *   3. per plane, last to first: rtxpt_b200_denoiser_prepare_inputs (own tiles); exchange the seven RTXPT_BUFFER_DENOISER_* / COMBINED_HISTORY_CLAMP_RELAX images;
  *      rtxpt_b200_reblur_denoise (whole frame, replicated: every rank keeps the same history); rtxpt_b200_denoiser_final_merge (own tiles)
  *   4. exchange { OUTPUT_COLOR_F16 }; rtxpt_b200_tone_map                                    auto exposure reads the whole frame
+ * With DLSS-RR instead of ReBLUR, steps 3 and 4 become: rtxpt_b200_dlss_rr_prepare_inputs (own tiles); exchange { OUTPUT_COLOR_F16, RR_DIFFUSE_ALBEDO_R11G11B10,
+ * RR_SPECULAR_ALBEDO_R11G11B10, RR_NORMALS_ROUGHNESS_F16, RR_SPECULAR_MOTION_VECTORS_F16 }: every rank then holds the whole RR set; DLSS-RR
+ * also reads the whole frame's DEPTH_F32 (step 2's set) and MOTION_VECTORS_F16 (add it to step 2's set).
  * exchange = rtxpt_b200_exchange_pack into a send buffer of rtxpt_b200_exchange_bytes bytes, ncclAllGather (or torch.distributed.all_gather_into_tensor) into
  * tileWorld x that many bytes, rtxpt_b200_exchange_unpack.  With NEEATFeedback = 0 the assembled frame is bit-identical to the single-GPU frame (tests/test_gpu_multi.py); with
  * feedback every rank adapts on its own tiles (independent global tables, local samplers clamped at screen-tile borders: still unbiased, SURVEY §8e). */

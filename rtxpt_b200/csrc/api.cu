@@ -5,6 +5,7 @@
 // There is no CPU rendering fallback anywhere in this library: without a CUDA device every entry point fails with RTXPT_ERR_NO_DEVICE.
 #include "kernels.h"
 #include "debug_views.cuh"
+#include "denoiser_iface.cuh"
 #include "opacity_masks.h"
 #include "reblur_host.h"
 #include "neeat_host.h"
@@ -162,6 +163,9 @@ struct rtxpt_ctx
     // denoiser interface: NRD's inputs for one plane at a time (allocated by the first prepare_inputs call)
     DeviceArray<float> dnViewZ; DeviceArray<uint2> dnMotion, dnDiff, dnSpec; DeviceArray<uint32_t> dnNormalRoughness; DeviceArray<uint8_t> dnDisocclusionMix, dnHistoryClampRelax;
     uint32_t denoiserWidth = 0, denoiserHeight = 0;
+    uint32_t realtimeFrameWidth = 0, realtimeFrameHeight = 0;         // image size of the last rtxpt_b200_path_trace_realtime (0: none yet)
+    // DLSS-RR inputs (rtxpt_b200_dlss_rr_prepare_inputs): R11G11B10 diffuse / specular albedo, RGBA16F normals + roughness, RG16F specular motion vectors; allocated by the first call
+    DeviceArray<uint32_t> rrDiffAlbedo, rrSpecAlbedo, rrSpecMotionVectors; DeviceArray<uint2> rrNormalsRoughness; uint32_t rrWidth = 0, rrHeight = 0;
     DeviceArray<float> dnScratchFloat;          // ping-pong partner of the specular hit distance guide (DenoiseSpecHitT)
     // ReBLUR: one permanent pool per stable plane (RTXPT keeps one NRD instance per plane, Sample.cpp:2560-2618), one transient pool and one pair of outputs shared by all
     struct ReblurHistory
@@ -920,6 +924,7 @@ extern "C" RTXPT_API int rtxpt_b200_set_realtime(rtxpt_ctx* c, const RtxptRealti
         CU(c->stablePlanes.alloc(planeStride * RTXPT_STABLE_PLANE_COUNT)); CU(c->stablePlanesHeader.alloc(P * 4)); CU(c->stableRadiance.alloc(P)); CU(c->specularHitT.alloc(P));
         CU(c->stablePlanes.fill(0, c->stream)); CU(c->stablePlanesHeader.fill(0xFF, c->stream)); CU(c->stableRadiance.fill(0, c->stream)); CU(c->specularHitT.fill(0, c->stream));
         c->realtimeWidth = W; c->realtimeHeight = H;
+        c->realtimeFrameWidth = c->realtimeFrameHeight = 0;        // the new planes hold no frame yet
     }
     c->realtime = *rt; c->haveRealtime = true;
     return RTXPT_OK;
@@ -1010,6 +1015,7 @@ extern "C" RTXPT_API int rtxpt_b200_path_trace_realtime(rtxpt_ctx* c, int mergeN
     CU(cudaEventRecord(c->evStop, s));
     CU(cudaMemcpyAsync(c->hCounters, c->counters.ptr, kCounterWords * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     c->lastIterations = fillIterations; c->lastSubSamples = 1; c->lastLaunches = launches; c->lastLanes = 1; c->lastSubSamplesPerLaunch = 1; c->statsPending = true;
+    c->realtimeFrameWidth = c->tableWidth; c->realtimeFrameHeight = c->tableHeight;
     return RTXPT_OK;
 }
 
@@ -1043,6 +1049,27 @@ extern "C" RTXPT_API int rtxpt_b200_denoiser_prepare_inputs(rtxpt_ctx* c, uint32
     LaunchParams p; fillParams(c, p); fillRealtimeParams(c, p);
     p.rt.dn = *k; p.rt.dnPlane = stablePlaneIndex; p.rt.dnInitWithStableRadiance = initWithStableRadiance ? 1u : 0u;
     launchDnPrepareInputs(p, c->grid, s);
+    CU(cudaGetLastError());
+    return RTXPT_OK;
+}
+// PostProcess DLSSRRDenoiserPrepareInputs (PostProcess.hlsl:175-440, Sample.cpp:2710-2757): the stable planes into the images DLSS Ray Reconstruction reads
+extern "C" RTXPT_API int rtxpt_b200_dlss_rr_prepare_inputs(rtxpt_ctx* c, float brightnessClampK, void* cudaStream)
+{
+    int rc = checkRealtimeReady(c); if (rc != RTXPT_OK) return rc;
+    if (c->realtimeFrameWidth != c->tableWidth || c->realtimeFrameHeight != c->tableHeight) return fail(RTXPT_ERR_INVALID_ARGUMENT, "no realtime frame at this image size: run rtxpt_b200_path_trace_realtime first");
+    if (!(std::isfinite(brightnessClampK) && brightnessClampK > 0.0f)) return fail(RTXPT_ERR_INVALID_ARGUMENT, "DLSSRRBrightnessClampK must be finite and positive (RTXPT's default is 4096)");
+    cudaStream_t s = pickStream(c, cudaStream);
+    if (c->rrWidth != c->tableWidth || c->rrHeight != c->tableHeight)
+    {
+        CU(syncContext(c));
+        const size_t P = size_t(c->tableWidth) * c->tableHeight;
+        CU(c->rrDiffAlbedo.alloc(P)); CU(c->rrSpecAlbedo.alloc(P)); CU(c->rrNormalsRoughness.alloc(P)); CU(c->rrSpecMotionVectors.alloc(P));
+        CU(c->rrDiffAlbedo.fill(0, s)); CU(c->rrSpecAlbedo.fill(0, s)); CU(c->rrNormalsRoughness.fill(0, s)); CU(c->rrSpecMotionVectors.fill(0, s));
+        c->rrWidth = c->tableWidth; c->rrHeight = c->tableHeight;
+    }
+    LaunchParams p; fillParams(c, p); fillRealtimeParams(c, p);
+    const DlssRrTargets rr{ c->rrDiffAlbedo.ptr, c->rrSpecAlbedo.ptr, c->rrNormalsRoughness.ptr, c->rrSpecMotionVectors.ptr, brightnessClampK };
+    launchDnPrepareDlssRr(p, rr, c->grid, s);
     CU(cudaGetLastError());
     return RTXPT_OK;
 }
@@ -1711,6 +1738,13 @@ static int targetInfo(rtxpt_ctx* c, int buffer, void** ptr, size_t* bytes)
     case RTXPT_BUFFER_DEBUG_VIZ_F16:
         if (c->debugViz.count != P) return fail(RTXPT_ERR_INVALID_ARGUMENT, "the debug view target does not exist before a path_trace call with a debug view set");
         *ptr = c->debugViz.ptr; *bytes = P * 8; return RTXPT_OK;
+    case RTXPT_BUFFER_RR_DIFFUSE_ALBEDO_R11G11B10: case RTXPT_BUFFER_RR_SPECULAR_ALBEDO_R11G11B10: case RTXPT_BUFFER_RR_NORMALS_ROUGHNESS_F16: case RTXPT_BUFFER_RR_SPECULAR_MOTION_VECTORS_F16:
+        if (c->rrWidth != c->tableWidth || c->rrHeight != c->tableHeight) return fail(RTXPT_ERR_INVALID_ARGUMENT, "the DLSS-RR inputs do not exist before rtxpt_b200_dlss_rr_prepare_inputs");
+        if (buffer == RTXPT_BUFFER_RR_DIFFUSE_ALBEDO_R11G11B10) { *ptr = c->rrDiffAlbedo.ptr; *bytes = P * 4; }
+        else if (buffer == RTXPT_BUFFER_RR_SPECULAR_ALBEDO_R11G11B10) { *ptr = c->rrSpecAlbedo.ptr; *bytes = P * 4; }
+        else if (buffer == RTXPT_BUFFER_RR_NORMALS_ROUGHNESS_F16) { *ptr = c->rrNormalsRoughness.ptr; *bytes = P * 8; }
+        else { *ptr = c->rrSpecMotionVectors.ptr; *bytes = P * 4; }
+        return RTXPT_OK;
     case RTXPT_BUFFER_LDR_COLOR_RGBA8:
         if (!c->toneMapped || c->ldrColor.count != P) return fail(RTXPT_ERR_INVALID_ARGUMENT, "the LDR colour does not exist before rtxpt_b200_tone_map");
         *ptr = c->ldrColor.ptr; *bytes = P * 4; return RTXPT_OK;

@@ -153,4 +153,119 @@ PT_HD void dnFinalMergeDebugPixel(const LaunchParams& p, const uint id)
     p.dbg.viz[size_t(ty) * W + tx] = packDebugPixel(mergeDebugColor(p.dbg.view, m));
 }
 
+// ---- DENOISER_DLSS_RR (PostProcess.hlsl:198-411): the images RTXPT hands DLSS Ray Reconstruction (TagResourcesDLSSRR, Sample.cpp:2710-2757) ----------------------------------
+// Formats (RenderTargets.cpp:185-197): OutputColor RGBA16F (p.outputColor), RRDiffuseAlbedo / RRSpecAlbedo R11G11B10_FLOAT, RRNormalsAndRoughness RGBA16F, RRSpecMotionVectors RG16F.
+// The targets reach k_dn_prepare_dlss_rr as an argument of their own, so that LaunchParams, and with it every other kernel, keeps its layout.
+struct DlssRrTargets { uint* diffAlbedo; uint* specAlbedo; uint2* normalsRoughness; uint* specMotionVectors; float brightnessClampK; };
+
+// what the pass computes for a pixel before the stores convert it; specMotionFromGuide: the pixel keeps u_MotionVectors.xy, whose fp16 halves are stored as they are
+struct DlssRrPixel { float3 color, diffAlbedo, specAlbedo, normal; float roughness; float2 specMotion; bool specMotionFromGuide; };
+
+// ComputeSpecularMotionVector (PostProcess.hlsl:94-160, the clipToWindowScale branch): the reflection hit mirrored behind a planar reflector, camera motion only
+PT_HD float2 computeSpecularMotionVector(const RealtimeParams& rt, float3 primaryHitPos, float3 primaryRayDir, float3 primaryHitNormal, float3 reflectionRay)
+{
+    float3 principalAxis = primaryHitNormal;
+    float zObj = dot3(principalAxis, reflectionRay);
+    if (zObj < 0.0f) { principalAxis = -principalAxis; zObj = -zObj; }
+    zObj = fmaxf(zObj, 1e-5f);
+    const float3 n = principalAxis;                                 // Duff et al., "Building an Orthonormal Basis, Revisited"
+    const float s = n.z < 0.0f ? -1.0f : 1.0f;
+    const float a = -1.0f / (s + n.z);
+    const float b = n.x * n.y * a;
+    const float3 xAxis = mk3(1.0f + s * n.x * n.x * a, s * b, -s * n.x);
+    const float3 yAxis = mk3(b, s + n.y * n.y * a, -n.y);
+    const float3 image = mk3(dot3(xAxis, reflectionRay), dot3(yAxis, reflectionRay), -zObj);
+    const float3 w = primaryHitPos + primaryRayDir * len3(image);
+    const float* Q = rt.prevWorldToClipNoOffset; const float* M = rt.worldToClipNoOffset;      // float4(w, 1) x matrix
+    const float qx = ((w.x * Q[0] + w.y * Q[4]) + w.z * Q[8]) + Q[12], qy = ((w.x * Q[1] + w.y * Q[5]) + w.z * Q[9]) + Q[13], qw = ((w.x * Q[3] + w.y * Q[7]) + w.z * Q[11]) + Q[15];
+    const float cx = ((w.x * M[0] + w.y * M[4]) + w.z * M[8]) + M[12], cy = ((w.x * M[1] + w.y * M[5]) + w.z * M[9]) + M[13], cw = ((w.x * M[3] + w.y * M[7]) + w.z * M[11]) + M[15];
+    return mk2((qx / qw - cx / cw) * rt.clipToWindowScale[0], (qy / qw - cy / cw) * rt.clipToWindowScale[1]);
+}
+
+// DENOISER_DLSS_RR for pixel `id`, in the shader's order of operations (MIX_STABLE_RADIANCE, MIX_BY_THROUGHPUT and ALLOW_MIX_NORMALS on, as RTXPT ships it)
+PT_HD DlssRrPixel dlssRrPixel(const LaunchParams& p, const uint id, const float brightnessClampK)
+{
+    const size_t o = pixelOffset(p, id);
+    const uint planeCount = p.rt.activePlaneCount, dominant = headerWord(p, id, 3) & 3u;
+    DlssRrPixel r;
+    const uint2 sr = p.rt.stableRadiance[o];
+    r.color = mk3(f16tof32(sr.x), f16tof32(sr.x >> 16), f16tof32(sr.y));
+    float3 stableAlbedo;
+    {   // sqrt(ReinhardMax(stable radiance)) (Utils.hlsli:85-90)
+        const float m = fmaxf(1e-7f, fmaxf(fmaxf(r.color.x, r.color.y), r.color.z));
+        const float reinhard = m / (m + 1);
+        const float3 t = r.color * (reinhard / m);
+        stableAlbedo = mk3(sqrtf(t.x), sqrtf(t.y), sqrtf(t.z));
+    }
+    const float stableAlbedoAvg = average(stableAlbedo);
+    float3 guideNormals = mk3(0.0f, 0.0f, 1e-6f), diffAlbedo = mk3(0.0f), specAlbedo = mk3(0.0f);
+    float roughness = 0.0f;
+    float w[3];
+    {   // plane weights: throughput 0.2, equalisation 0.01, dominant plane +0.05; planes without a branch drop out (plane 0 always counts), then normalised
+        float thp[3] = { 1.0f, 0.0f, 0.0f }, available[3] = { 1.0f, 0.0f, 0.0f };
+        for (uint i = 1; i < planeCount; i++)
+        {
+            if (headerWord(p, id, i) == kInvalidBranchID) continue;
+            const uint4 r2 = reinterpret_cast<const uint4*>(p.rt.planes + planeAddress(p.rt, id, i))[2];
+            const float weight = sat(average(mk3(f16tof32(r2.x >> 16), f16tof32(r2.y >> 16), f16tof32(r2.z >> 16))));
+            thp[i] = weight; thp[0] = sat(thp[0] - weight); available[i] = 1.0f;
+        }
+        for (int k = 0; k < 3; k++) w[k] = (0.0f + thp[k] * 0.2f) + 0.01f;
+        if (dominant < 3u) w[dominant] += 0.05f;
+        for (int k = 0; k < 3; k++) w[k] *= available[k];
+        const float sum = w[0] + w[1] + w[2];
+        for (int k = 0; k < 3; k++) w[k] /= sum;
+    }
+    for (uint i = 0; i < planeCount; i++)
+    {
+        if (headerWord(p, id, i) == kInvalidBranchID) continue;
+        const uint4* rec = reinterpret_cast<const uint4*>(p.rt.planes + planeAddress(p.rt, id, i));
+        if (!isfinite(bitsToFloat(rec[1].w))) continue;                                     // skip sky
+        const uint4 r4 = rec[4];
+        r.color = r.color + mk3(f16tof32(r4.x), f16tof32(r4.x >> 16), f16tof32(r4.y));
+        const float weight = w[i];
+        if (weight > 1e-6f)
+        {
+            const uint4 r2 = rec[2], r3 = rec[3];
+            guideNormals = guideNormals + weight * octUnorm32ToDir(r3.w);
+            roughness = roughness + weight * f16tof32(r2.w);
+            diffAlbedo = diffAlbedo + weight * mk3(f16tof32(r3.x >> 16), f16tof32(r3.y >> 16), f16tof32(r3.z >> 16));
+            specAlbedo = specAlbedo + weight * mk3(f16tof32(r3.x), f16tof32(r3.y), f16tof32(r3.z));
+        }
+    }
+    const float3 stableAlbedoGreyMix = lerp3(stableAlbedo, mk3(0.5f), 0.2f);
+    diffAlbedo = lerp3(diffAlbedo, stableAlbedoGreyMix, stableAlbedoAvg / (average(diffAlbedo) + sqrtf(stableAlbedoAvg) + 1e-7f));
+    const float guideNormalsLength = len3(guideNormals);
+    r.normal = guideNormalsLength < 1e-5f ? mk3(0.0f, 0.0f, 1.0f) : mk3(guideNormals.x / guideNormalsLength, guideNormals.y / guideNormalsLength, guideNormals.z / guideNormalsLength);
+    if (average(diffAlbedo + specAlbedo) < 0.05f) diffAlbedo = diffAlbedo + mk3(0.05f);
+    const float maxRadiance = maxComp(r.color);
+    if (maxRadiance > brightnessClampK) r.color = r.color * (brightnessClampK / maxRadiance);
+    r.diffAlbedo = diffAlbedo; r.specAlbedo = specAlbedo; r.roughness = roughness;
+    {   // specular motion vectors from plane 0's hit and the specular hit distance; the roughness test reads the mixed guide roughness
+        const uint4* rec = reinterpret_cast<const uint4*>(p.rt.planes + planeAddress(p.rt, id, 0));
+        const uint4 r0 = rec[0], r1 = rec[1];
+        const float3 rayOrigin = mk3(bitsToFloat(r0.x), bitsToFloat(r0.y), bitsToFloat(r0.z)), rayDir = mk3(bitsToFloat(r1.x), bitsToFloat(r1.y), bitsToFloat(r1.z));
+        const float3 primaryHitPos = rayOrigin + rayDir * bitsToFloat(r1.w);
+        const float3 normal = octUnorm32ToDir(rec[3].w);
+        const float specHitT = p.rt.specularHitT[o];
+        const float3 reflectionRay = (rayDir - (2.0f * dot3(normal, rayDir)) * normal) * specHitT;       // reflect(dir, normal) * specHitT
+        r.specMotionFromGuide = !(specHitT > 1e-3f && roughness < 0.25f);                          // PathTracer::kSpecularRoughnessThreshold
+        if (r.specMotionFromGuide) { const uint g = p.motionVectors[o].x; r.specMotion = mk2(f16tof32(g), f16tof32(g >> 16)); }
+        else r.specMotion = computeSpecularMotionVector(p.rt, primaryHitPos, rayDir, normal, reflectionRay);
+    }
+    return r;
+}
+
+// the pass's stores.  R11G11B10: packR11G11B10, the rounding of every R11G11B10 store in the library; no reference source pins the conversion the hardware does on a UAV store
+PT_HD void dnPrepareDlssRrPixel(const LaunchParams& p, const DlssRrTargets& rr, const uint id)
+{
+    const DlssRrPixel r = dlssRrPixel(p, id, rr.brightnessClampK);
+    const size_t o = pixelOffset(p, id);
+    p.outputColor[o] = packRGBA16F(r.color.x, r.color.y, r.color.z, 1.0f);
+    rr.diffAlbedo[o] = packR11G11B10(r.diffAlbedo);
+    rr.specAlbedo[o] = packR11G11B10(r.specAlbedo);
+    rr.normalsRoughness[o] = packRGBA16F(r.normal.x, r.normal.y, r.normal.z, r.roughness);
+    rr.specMotionVectors[o] = r.specMotionFromGuide ? p.motionVectors[o].x : (f32tof16(r.specMotion.x) | (f32tof16(r.specMotion.y) << 16));
+}
+
 } // namespace pt

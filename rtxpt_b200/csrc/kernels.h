@@ -30,6 +30,8 @@ void launchRtMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchRtDebugViz(const LaunchParams& p, const GridConfig& g, cudaStream_t s);          // StablePlanesDebugViz after the FILL passes (rtxpt_b200_set_debug_view)
 void launchDnPrepareInputs(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchDnFinalMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
+struct DlssRrTargets;
+void launchDnPrepareDlssRr(const LaunchParams& p, const DlssRrTargets& rr, const GridConfig& g, cudaStream_t s);     // DENOISER_DLSS_RR (denoiser_iface.cuh)
 void launchCommitAccumulate(const LaunchParams& p, const GridConfig& g, cudaStream_t s);
 void launchTraceRays(const LaunchParams& p, const GridConfig& g, const RtxptRay* dRays, uint32_t count, bool anyHit, RtxptHit* dHits, uint32_t* dCounters, uint32_t* dCursor, cudaStream_t s);
 void launchPackOwned(const float4* image, const uint32_t* pixelOfSlot, uint32_t pixelCount, uint32_t paddedCount, uint32_t width, float4* dst, const GridConfig& g, cudaStream_t s);

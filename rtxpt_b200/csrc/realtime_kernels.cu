@@ -242,6 +242,11 @@ __global__ void __launch_bounds__(256) k_dn_final_merge(const __grid_constant__ 
         if constexpr (DEBUG_VIEW) dnFinalMergeDebugPixel(p, p.wf.pixelOfSlot[slot]);
     }
 }
+// DENOISER_DLSS_RR: one thread per owned pixel; the DLSS-RR targets are an argument of their own (denoiser_iface.cuh)
+__global__ void __launch_bounds__(256) k_dn_prepare_dlss_rr(const __grid_constant__ LaunchParams p, const DlssRrTargets rr)
+{
+    for (uint slot = blockIdx.x * blockDim.x + threadIdx.x; slot < p.wf.pixelCount; slot += gridDim.x * blockDim.x) dnPrepareDlssRrPixel(p, rr, p.wf.pixelOfSlot[slot]);
+}
 // DenoiseSpecHitT: one thread per pixel over the full frame (row-major guides); src / dst alternate between the guide and a scratch image
 __global__ void __launch_bounds__(256) k_dn_spec_hitt(const float* __restrict__ src, const float* __restrict__ depth, float* __restrict__ dst, int W, int H)
 {
@@ -283,6 +288,7 @@ void launchRtUnpackPlaneGuides(const LaunchParams& p, const uint32_t* allPixelTa
 { k_rt_unpack_plane_guides<<<g.smCount * 4, 256, 0, s>>>(p, allPixelTable, paddedCount, world, skipRank, static_cast<const uint8_t*>(srcAll), segmentOffset, bytesPerRank); }
 void launchDnSpecHitT(const float* src, const float* depth, float* dst, int W, int H, cudaStream_t s) { k_dn_spec_hitt<<<dim3((W + 15) / 16, (H + 15) / 16), dim3(16, 16), 0, s>>>(src, depth, dst, W, H); }
 void launchDnPrepareInputs(const LaunchParams& p, const GridConfig& g, cudaStream_t s) { k_dn_prepare_inputs<<<g.smCount * 4, 256, 0, s>>>(p); }
+void launchDnPrepareDlssRr(const LaunchParams& p, const DlssRrTargets& rr, const GridConfig& g, cudaStream_t s) { k_dn_prepare_dlss_rr<<<g.smCount * 4, 256, 0, s>>>(p, rr); }
 void launchDnFinalMerge(const LaunchParams& p, const GridConfig& g, cudaStream_t s)
 {
     if (p.dbg.viz && isDenoiserMergeView(p.dbg.view)) k_dn_final_merge<true><<<g.smCount * 4, 256, 0, s>>>(p); else k_dn_final_merge<<<g.smCount * 4, 256, 0, s>>>(p);

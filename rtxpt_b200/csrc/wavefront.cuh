@@ -391,9 +391,9 @@ PT_HD void computeCameraRay(const RtxptPathTracerConstants& c, uint id, uint sam
 
 // guide export (Bridge::ExportSurface / ExportNonSurface, BridgeDonut:1105-1146): only the last sub-sample of a launch writes, as the
 // reference's sequential sub-sample dispatches leave the last one in the buffers
-PT_DEVICE uint packR11G11B10(float3 rgb)        // Utils/Packing.hlsli:175-184
+PT_HD uint packR11G11B10(float3 rgb)            // Utils/Packing.hlsli:175-184
 {
-    const float top = __uint_as_float(0x477C0000u);
+    const float top = bitsToFloat(0x477C0000u);
     const uint r = ((f32tof16(fminf(rgb.x, top)) + 8u) >> 4) & 0x000007FFu;
     const uint g = ((f32tof16(fminf(rgb.y, top)) + 8u) << 7) & 0x003FF800u;
     const uint b = ((f32tof16(fminf(rgb.z, top)) + 16u) << 17) & 0xFFC00000u;

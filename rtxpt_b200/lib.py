@@ -55,6 +55,7 @@ _SIGNATURES = {
     "rtxpt_b200_path_trace_realtime": [C.c_void_p, C.c_int, C.c_void_p],
     "rtxpt_b200_denoiser_prepare_inputs": [C.c_void_p, C.c_uint32, C.c_int, C.POINTER(S.DenoiserConstants), C.c_void_p],
     "rtxpt_b200_denoiser_final_merge": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p],
+    "rtxpt_b200_dlss_rr_prepare_inputs": [C.c_void_p, C.c_float, C.c_void_p],
     "rtxpt_b200_skin_register": [C.c_void_p, C.POINTER(S.SkinDesc), C.POINTER(C.c_uint32)],
     "rtxpt_b200_skin_update": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p],
     "rtxpt_b200_tone_map": [C.c_void_p, C.POINTER(S.ToneMappingParams), C.c_int, C.c_void_p],
@@ -117,6 +118,13 @@ def load(strict=None):
         L.rtxpt_b200_default_constants.argtypes = [C.POINTER(S.CameraData), C.c_int, C.POINTER(S.PathTracerConstants)]; L.rtxpt_b200_default_constants.restype = C.c_int
         _libs[strict] = L
     return _libs[strict]
+
+
+def unpack_r11g11b10(words):
+    """R11G11B10_FLOAT words -> float32 [..., 3] (unsigned 11 / 11 / 10-bit floats: 5-bit exponent, fp16's bias)."""
+    w = np.asarray(words, np.uint32)
+    halves = [((w & 0x7FF) << 4), (((w >> 11) & 0x7FF) << 4), (((w >> 22) & 0x3FF) << 5)]
+    return np.stack([h.astype(np.uint16).view(np.float16).astype(np.float32) for h in halves], -1)
 
 
 def _check(rc, L=None):
@@ -386,6 +394,23 @@ class Context:
             if d_diff is None: d_diff = self.device_ptr(S.BUFFER_DENOISER_DIFF_RADIANCE_HITDIST_F16)[0]
             if d_spec is None: d_spec = self.device_ptr(S.BUFFER_DENOISER_SPEC_RADIANCE_HITDIST_F16)[0]
         _check(self.L.rtxpt_b200_denoiser_final_merge(self.h, plane, d_diff, d_spec, stream), self.L)
+
+    # ---- DLSS Ray Reconstruction's inputs ----
+    def dlss_rr_prepare_inputs(self, brightness_clamp_k=S.DLSS_RR_BRIGHTNESS_CLAMP_K, stream=None):
+        """PostProcess DLSSRRDenoiserPrepareInputs: after path_trace_realtime(merge_no_denoiser=False) and denoise_spec_hit_t.  brightness_clamp_k is the shader constant
+        PathTracerConstants::DLSSRRBrightnessClampK = the UI value (4096) x preExposedGrayLuminance (Sample.cpp:1526); the default holds without tone mapping."""
+        _check(self.L.rtxpt_b200_dlss_rr_prepare_inputs(self.h, float(brightness_clamp_k), stream), self.L)
+
+    def readback_dlss_rr(self):
+        """The DLSS-RR set: color float16 [H, W, 4] (the output colour), diff_albedo / spec_albedo uint32 [H, W] R11G11B10 words (unpack_r11g11b10 decodes them),
+        normals_roughness float16 [H, W, 4], spec_motion float16 [H, W, 2]."""
+        h, w = self.consts.imageHeight, self.consts.imageWidth
+        out = dict(color=self.readback_output_color(), diff_albedo=np.empty((h, w), np.uint32), spec_albedo=np.empty((h, w), np.uint32),
+                   normals_roughness=np.empty((h, w, 4), np.float16), spec_motion=np.empty((h, w, 2), np.float16))
+        for key, buf in (("diff_albedo", S.BUFFER_RR_DIFFUSE_ALBEDO_R11G11B10), ("spec_albedo", S.BUFFER_RR_SPECULAR_ALBEDO_R11G11B10),
+                         ("normals_roughness", S.BUFFER_RR_NORMALS_ROUGHNESS_F16), ("spec_motion", S.BUFFER_RR_SPECULAR_MOTION_VECTORS_F16)):
+            _check(self.L.rtxpt_b200_readback(self.h, buf, out[key].ctypes.data, out[key].nbytes), self.L)
+        return out
 
     def skin_register(self, instance, geometry, positions, joint_indices, joint_weights, normals=None, tangents=None):
         """Bind pose of one geometry (vertex order of its vertex buffer); returns the skin id for skin_update."""

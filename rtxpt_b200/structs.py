@@ -42,7 +42,9 @@ BUFFER_DENOISED_DIFF_RADIANCE_HITDIST_F16, BUFFER_DENOISED_SPEC_RADIANCE_HITDIST
 BUFFER_LDR_COLOR_RGBA8 = 19
 BUFFER_STABLE_PLANE_NEIGHBOUR_GUIDES = 20        # exchange only (rtxpt_b200_exchange_*)
 BUFFER_DEBUG_VIZ_F16 = 21                        # rtxpt_b200_set_debug_view
-
+# DLSS-RR inputs (rtxpt_b200_dlss_rr_prepare_inputs)
+BUFFER_RR_DIFFUSE_ALBEDO_R11G11B10, BUFFER_RR_SPECULAR_ALBEDO_R11G11B10, BUFFER_RR_NORMALS_ROUGHNESS_F16, BUFFER_RR_SPECULAR_MOTION_VECTORS_F16 = 22, 23, 24, 25
+DLSS_RR_BRIGHTNESS_CLAMP_K = 4096.0              # PathTracerConstants::DLSSRRBrightnessClampK with RTXPT's UI default and tone mapping off; with it on, times preExposedGrayLuminance (Sample.cpp:1526)
 
 class GeometryData(C.Structure):
     _fields_ = [("numIndices", u32), ("numVertices", u32), ("indexBufferIndex", i32), ("indexOffset", u32),
